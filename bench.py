@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- frames/s of the 832x624 composite modulate + demodulate hot path on B200.
+"""bench.py -- frames/s of the 832x624 composite modulate + demodulate hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W            # product (CUDA) arm
     python bench.py --impl reference --gpus N ...            # reference C on the host cores
+    python bench.py ... --dump-outputs DIR                   # also save what the last timed step decoded (see dump_outputs)
 
 A "step" is one pass of the hot path over one batch: every monitor of the batch gets one
 crt_modulate + crt_demodulate pair (= one field = one "frame" of the metric, SURVEY.md 8d).
@@ -463,8 +464,8 @@ def config4_block(args, dev, rank, world, noise=0):
         return out
 
     frames = make_frames(lo, hi)
-    # time-parallel segments per rank: ~8 frames each (a two-frame halo on top), at most one line-kernel wave (296 monitors)
-    segs = args.config4_segments if args.config4_segments > 0 else max(16, min(296, (hi - lo) // 8))
+    # time-parallel segments per rank: ~8 frames each (a two-frame halo on top), at most one line-kernel wave (264 monitors)
+    segs = args.config4_segments if args.config4_segments > 0 else max(16, min(264, (hi - lo) // 8))
     segs = max(1, min(segs, hi - lo))
     conv = video.VideoConverter("ntsc", ow, oh, noise=noise, scanlines=1, segments=segs)
     if world > 1:
@@ -533,6 +534,21 @@ def config4_block(args, dev, rank, world, noise=0):
             "exchange": "all_gather of 2 input frames + sync state + last image per rank (seam verification), NCCL" if world > 1 else "none (one rank)",
             "bit_identical_to_sequential_loop": bool(flag == 0), "frames_checked": checked if rank == 0 else None,
             "sequential_loop_s_rank0": seq_s}
+
+
+def dump_outputs(path, out):
+    """--dump-outputs: the decoded images of the last timed step -- what a caller of crtx_modulate + crtx_demodulate
+    receives -- as .npy files of at most 64 MB in all, so that two builds can be compared output for output (the inputs
+    are seeded): four whole images chosen with a fixed seed (float32, [4, H, W, 4] BGRA) with their batch indices, and
+    the per-row, per-channel sums of every image of the batch (float64, [B, H, 4])."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    pick = np.sort(np.random.default_rng(0).choice(out.shape[0], size=min(4, out.shape[0]), replace=False))
+    sample = out[torch.as_tensor(pick, device=out.device)].cpu().numpy()
+    np.save(os.path.join(path, "images_sample.npy"), sample.astype(np.float32))
+    np.save(os.path.join(path, "images_sample_index.npy"), pick.astype(np.float64))
+    np.save(os.path.join(path, "row_channel_sums.npy"), out.sum(dim=2, dtype=torch.int64).cpu().numpy().astype(np.float64))
 
 
 def run_product(args):
@@ -625,6 +641,8 @@ def run_product(args):
     barrier()
     ms = ev0.elapsed_time(ev1)
     clocks = sampler.finish()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out)
     launches = batch.launches - launches0
     took_lines2 = batch.lines2_launches - lines2_0
     batch.set_option("timing", 1)
@@ -794,8 +812,8 @@ def run_product(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "fallback 3350 GB/s (H100 SXM data sheet, not measured)"
         lines_ms, lines_n = ktimes["lines"]
         sync_ms, sync_n = ktimes["sync"]
         noise_ms, _ = ktimes["noise"]
@@ -893,8 +911,8 @@ def main():
     ap.add_argument("--impl", default="product", choices=["product", "reference", "dropin"],
                     help="dropin: only the informational drop-in figure (used by the product arm in a child process)")
     ap.add_argument("--dropin-seconds", type=float, default=2.0)
-    ap.add_argument("--batch", type=int, default=296,
-                    help="monitors (frames per step) per GPU; 296 = 148 SMs x the two monitors a line-kernel CTA decodes")
+    ap.add_argument("--batch", type=int, default=264,
+                    help="monitors (frames per step) per GPU; 264 = 132 SMs of an H100 x the two monitors a line-kernel CTA decodes")
     ap.add_argument("--e2e-batch", type=int, default=128)
     ap.add_argument("--e2e-streams", type=int, default=4)
     ap.add_argument("--sustained-seconds", type=float, default=1.2, help="0: skip the sustained block")
@@ -905,6 +923,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-allgather", action="store_true", help="N > 1: skip the all_gather / gather_to_root blocks")
     ap.add_argument("--no-numa", action="store_true", help="do not bind the process to the GPU's NUMA node")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/*.npy")
     ap.add_argument("--variant", default="ntsc", choices=["ntsc", "ntsc_conv", "ntsc_conv6", "ntsc_conv5", "ntsc_conv4", "nes", "nes_p0", "nes_p1", "snes", "nesrgb", "nesrgb_p0", "nesrgb_p1", "vhs", "template", "pv1k", "ntsc_bloom"],
                     help="informational runs of the other systems (the contract metric is the default, ntsc)")
     args = ap.parse_args()

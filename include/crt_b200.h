@@ -7,7 +7,7 @@
  *   crt_bpp4fmt, crt_sincos14          crt_core.h:100-139
  * so the reference's unmodified C89 drivers (crt_main.c, extra/video_convert.c) compile
  * against it and link with lib/libcrt_b200_<variant>.so instead of crt_core.c + crt_<sys>.c
- * (see INTEGRATION.md).  Behind these entry points the work is done by sm_100a CUDA
+ * (see INTEGRATION.md).  Behind these entry points the work is done by sm_90a CUDA
  * kernels; there is no CPU implementation in the library.
  *
  * Like the reference, the interface is compile-time polymorphic: define CRT_SYSTEM

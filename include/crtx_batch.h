@@ -151,7 +151,7 @@ long crtx_lines2_count(crtx_ctx *ctx); /* of those, line passes taken by k_lines
                                          * stock IIR decoder on 4-byte pixels, 16-byte aligned images, outw a multiple of 4 in about
                                          * [528, 1312]); every other geometry runs k_lines.  For tests and A/B runs (option "lines2"). */
 /* options: "tma", "generic_eq", "timing", "mod_staged", "fused_noise", "mod_bulk", "lines2", "host_rows", "pdl" (0/1 switches; "pdl" 1 launches the
- * picture, sync and line kernels as programmatic dependents of their predecessors: measured no gain, default 0), "lines2_stage" (how k_lines2 stages
+ * picture, sync and line kernels as programmatic dependents of their predecessors, default 0), "lines2_stage" (how k_lines2 stages
  * the signal windows: 2 = cp.async, the default; 1 = one bulk copy per lane), "host_src" (1:
  * crtx_frames_host lets the encoder read page-locked source images in place instead of copying them), and
  * "line_lo" / "line_hi": crtx_demodulate's line pass only decodes scanlines [line_lo, line_hi) of every

@@ -1,10 +1,10 @@
-"""ntsc-crt_b200 -- B200-native composite modulate/demodulate hot path of NTSC-CRT.
+"""ntsc-crt_b200 -- H100-native composite modulate/demodulate hot path of NTSC-CRT.
 
 The directory name carries a hyphen (it is the project name); import it through
 `pkgload.load()` at the repo root, which registers it as module `ntsc_crt_b200`.
 
 Contents (only what the hot path needs):
-  csrc/      hand-written sm_100a CUDA kernels + the C-ABI (crt_* drop-in, crtx_* batch)
+  csrc/      hand-written sm_90a CUDA kernels + the C-ABI (crt_* drop-in, crtx_* batch)
   lib/       the built shared libraries, one per reference variant (git-ignored)
   layout.py  ctypes mirror of struct CRT / struct NTSC_SETTINGS
   capi.py    loader for the product libraries (fails loudly if they are missing)

@@ -1,4 +1,4 @@
-// crt_kernels.cuh -- the sm_100a kernels of the composite modulate -> noise -> demodulate path.
+// crt_kernels.cuh -- the sm_90a kernels of the composite modulate -> noise -> demodulate path.
 //
 // Kernel map (reference lines each one replaces):
 //   k_mod_skeleton_rgb  sync / blanking / burst skeleton of all 262 lines  crt_ntsc.c:205-252, 325-329
@@ -190,9 +190,8 @@ __device__ __forceinline__ void mod_skeleton_prime(const SrcCfg &s, MonState *st
     if (kIsVhs && e == 0) st->hsync = 0; // crt_ntscvhs.c:258-259
 }
 
-// One CTA per monitor.  (Round 2 tried carrying this work on a ninth warp of the staged picture kernel: 155 us against
-// 21 + 130 separately, and the picture of a line shifted right by xoffset >= 4 spills three bytes into the next line's
-// porch, which the reference's write order resolves -- dropped.)
+// One CTA per monitor.  (Not folded into the staged picture kernel as a ninth warp: the picture of a line shifted right
+// by xoffset >= 4 spills three bytes into the next line's porch, which the reference's write order resolves.)
 __global__ void __launch_bounds__(256) k_mod_skeleton_rgb(const SrcCfg *__restrict__ srcs,
                                                           MonState *__restrict__ states,
                                                           signed char *__restrict__ analog_base, int first)
@@ -388,7 +387,7 @@ constexpr int kModSChunk = 32;                     // samples per chunk
 constexpr int kModSSpan = 192;                     // largest staged span the kernel accepts (incl. alignment slack)
 // Stage bytes per line per chunk.  Every lane reads "its row, same column" at once, and rows start on
 // 16-byte boundaries, so the pitch decides the bank conflicts: 192 B (48 words) put all 32 lanes on 2
-// banks (16-way, measured as the top stall of this kernel); 176 B (44 words) spreads them over 8 (4-way,
+// banks (16-way); 176 B (44 words) spreads them over 8 (4-way,
 // the best a 16-byte granular pitch can do).  176 is also exactly the largest copy an accepted span needs.
 constexpr int kModSRow = 176;
 constexpr int kModSOutPitch = kModSChunk / 4 + 1;  // words

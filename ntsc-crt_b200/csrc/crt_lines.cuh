@@ -78,8 +78,8 @@ __device__ __forceinline__ int eq_step(Eq &f, int s, int rnd)
     return r;
 }
 
-// crt_core.c:573-581 -> 0x00RRGGBB.  (Measured on B200: issuing the shifts as IMAD.HI and the clamps as
-// I2I.SAT to unload the ALU pipe made the kernel 7 % slower -- both are slower-rate instructions.)
+// crt_core.c:573-581 -> 0x00RRGGBB.  (Shifts and clamps stay on the ALU pipe: IMAD.HI and I2I.SAT are slower-rate
+// instructions.)
 // HALF: every channel already halved, as the blend needs it -- floor(clamp(v >> 8, 0, 255) / 2) == clamp(v >> 9, 0, 127)
 template <bool HALF = false>
 __device__ __forceinline__ unsigned yiq_to_rgb(int y, int i, int q, int contrast)
@@ -355,8 +355,8 @@ k_lines(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, co
     };
     auto get = [&](const unsigned char *p, int &cy, int &ci, int &cq) {
         if (FAST) {
-            // (16-bit sign-extending loads of the halves instead of this unpacking were measured 3 % slower
-            // here: per-lane rows make them 2-way bank conflicted)
+            // (one 8-byte load and an unpacking rather than 16-bit sign-extending loads of the halves: per-lane
+            // rows make those 2-way bank conflicted)
             const uint2 v = *reinterpret_cast<const uint2 *>(p);
             cy = (int) v.x;
             ci = (int) (short) (unsigned short) v.y; // sign-extended low half

@@ -4,8 +4,7 @@
 // very narrow or very wide outputs, the wrap-exact generic equaliser, rows shared by several lines, the PV-1000 --
 // stays with k_lines (crt_lines.cuh); the host picks per launch (crtx.cu: lines2_eligible).
 //
-// Same shape as k_lines -- one LANE carries one scanline through the equalisers -- with the three things its
-// profile asked for (profiles/r1_source_view_notes.md, VERDICT r1 "what's weak" 1-3):
+// Same shape as k_lines -- one LANE carries one scanline through the equalisers -- with three changes:
 //   * a CTA is 15 warps = 480 lane-lines = TWO monitors.  240 lines are 7.5 warps: k_lines leaves half a warp
 //     empty per monitor (1/16 of all issued instructions);
 //   * the resampler's index arithmetic is gone from the instruction stream.  Which two samples pixel k reads and

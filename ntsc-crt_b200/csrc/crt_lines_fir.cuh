@@ -114,7 +114,7 @@ k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states
     const int stride = (int) gridDim.x * kFirWarps;
 
     // A record is fetched two lines before it is decoded and must not be LOOKED AT before it is needed:
-    // deciding "active" at fetch time made every line wait for this load (5 % of the kernel's samples).
+    // deciding "active" at fetch time would make every line wait for this load.
     auto fetch = [&](int kl) -> FirLine { // warp-uniform
         FirLine l;
         l.pos = l.wave0 = l.wave1 = l.run_pos = l.run_last = 0;
@@ -296,8 +296,8 @@ k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states
                 if (FAST) {
                     const int L4 = 0x3ffc - R4; // 4 * L
                     const int y = wadd(wmul(ay, L4), wmul(by, R4));
-                    // (v * 4L) >> 16 == (v * L) >> 14: the two dropped bits are zeros.  (One IMAD.HI per term instead
-                    // of multiply + shift was measured 3 % SLOWER on B200: IMAD.HI is a multi-pass instruction.)
+                    // (v * 4L) >> 16 == (v * L) >> 14: the two dropped bits are zeros.  (Multiply + shift rather than one
+                    // IMAD.HI per term: IMAD.HI is a multi-pass instruction.)
                     return yiq_to_rgb<MODE == 1>(y, wadd(wmul(ai, L4) >> 16, wmul(bi, R4) >> 16),
                                                  wadd(wmul(aq, L4) >> 16, wmul(bq, R4) >> 16), contrast);
                 } else {

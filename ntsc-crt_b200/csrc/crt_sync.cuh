@@ -27,7 +27,7 @@ constexpr int kCandWords = (kHres + 3) / 4 + 1;                     // a whole l
 // One head more than there are signal lines: with hsync in the second half of a line (the steady state of the
 // NTSC timing, ~898) the search window of the LAST signal line sits on the start of the line after it.  Those
 // bytes are the padding after inp[] (the reference reads past its array there); staging them keeps that one
-// line off the 16-dependent-loads fall-back, which used to hold every sweep's barrier for ~5 us.
+// line off the 16-dependent-loads fall-back, which would hold every sweep's barrier.
 constexpr int kHeadLines = kVres + 1;
 constexpr int kSyncSmem = (kHeadLines * kHeadWords + 2 * kVsyncWindow * kCandWords) * 4;
 constexpr int kSyncThreads = 256;
@@ -239,8 +239,8 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
 
     // ---- 1. stage line heads (heads[j][w] = the aligned word at ((j * H - 16) & ~3) + 4w) and the 2W
     // vsync candidate lines in full (cand[c][w] = aligned words covering line posmod(vsync + c - W)).  The signal is
-    // read in 16-byte vectors, kStageBatch of them in flight per thread (word-sized loads in batches of 8 spent 16 us here,
-    // most of it on index arithmetic), the noise applied, and the four words land at their places in the row.
+    // read in 16-byte vectors, kStageBatch of them in flight per thread (word-sized loads in batches would spend most of
+    // the time on index arithmetic), the noise applied, and the four words land at their places in the row.
     unsigned *cand = heads + kHeadLines * kHeadWords; // [2W][kCandWords]
     const int vs_in = st->vsync;
     // candidate c is line posmod(vsync + c - W, VRES) (crt->vsync is the caller's to poke: any value); one modulo per thread
@@ -354,8 +354,8 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
     __syncthreads();
     phase_mark(0, 3);
     // Decoded lines of each colour row, in order (skipped lines do not touch ccf).  Warp r compacts row r
-    // with ballots, 32 lines per step -- a 240-iteration loop on one thread per row here made every other
-    // thread wait ~13 % of the kernel at the next barrier.
+    // with ballots, 32 lines per step -- a 240-iteration loop on one thread per row here would make every other
+    // thread wait at the next barrier.
     if (warp < kVper) {
         int n = 0;
         for (int k0 = 0; k0 < kLines; k0 += 32) {

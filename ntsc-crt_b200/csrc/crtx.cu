@@ -758,12 +758,13 @@ int crtx_create(crtx_ctx **out, int n)
     CUDA_TRY(cudaGetDevice(&dev));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major < 10) return fail("crtx_create: device %d is sm_%d%d, this library is built for sm_100a only", dev, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        return fail("crtx_create: device %d is sm_%d%d, this library is built for sm_90a only", dev, prop.major, prop.minor);
 
     crtx_ctx *ctx = new crtx_ctx();
     ctx->n = n;
     ctx->device = dev;
-    ctx->sm_count = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 148;
+    ctx->sm_count = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 132;
     ctx->h_cfg.assign(n, MonCfg());
     memset(ctx->h_cfg.data(), 0, sizeof(MonCfg) * n);
     ctx->cfg_dirty_lo = 0;
@@ -1214,7 +1215,7 @@ int crtx_memcmp_device(const void *a, const void *b, size_t bytes, int *differ, 
     CUDA_TRY(cudaMalloc(&flag, sizeof(int)));
     cudaMemsetAsync(flag, 0, sizeof(int), (cudaStream_t) stream);
     const size_t words = bytes / 16;
-    k_differs<<<296, 256, 0, (cudaStream_t) stream>>>((const uint4 *) a, (const uint4 *) b, words,
+    k_differs<<<264, 256, 0, (cudaStream_t) stream>>>((const uint4 *) a, (const uint4 *) b, words,
                                                      (const unsigned char *) a + words * 16,
                                                      (const unsigned char *) b + words * 16, (int) (bytes - words * 16), flag);
     cudaError_t e = cudaMemcpyAsync(differ, flag, sizeof(int), cudaMemcpyDeviceToHost, (cudaStream_t) stream);
@@ -1276,7 +1277,7 @@ int crtx_fade_phosphors(void *image, size_t npix, void *stream)
     if (npix == 0) return 0;
     size_t blocks = (npix / 4 + 255) / 256;
     if (blocks < 1) blocks = 1;
-    if (blocks > 148 * 8) blocks = 148 * 8; // a few resident CTAs per SM, grid-stride beyond
+    if (blocks > 132 * 8) blocks = 132 * 8; // a few resident CTAs per SM of an H100, grid-stride beyond
     k_fade_phosphors<<<(unsigned) blocks, 256, 0, (cudaStream_t) stream>>>((unsigned *) image, npix);
     CUDA_TRY(cudaGetLastError());
     return 0;

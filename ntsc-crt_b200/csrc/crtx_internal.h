@@ -13,7 +13,7 @@
 struct crtx_ctx {
     int n = 0;
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     crt::MonCfg *d_cfg = nullptr;
     crt::MonState *d_state = nullptr;
     crt::SrcCfg *d_src = nullptr;
@@ -48,11 +48,11 @@ struct crtx_ctx {
     int opt_timing = 0;
     int opt_mod_staged = 1;
     int opt_fused_noise = 1;
-    int opt_mod_bulk = 1; // encoder staging: 1 = per-lane bulk copies, 0 = per-lane cp.async (A/B switch; measured equal)
-    int opt_pdl = 0;      // 1: programmatic dependent launch of picture / sync / line kernels behind their predecessors (measured: no gain -- every kernel is one wave that ends within microseconds across the SMs -- so ordinary launches are the default)
+    int opt_mod_bulk = 1; // encoder staging: 1 = per-lane bulk copies, 0 = per-lane cp.async (A/B switch)
+    int opt_pdl = 0;      // 1: programmatic dependent launch of picture / sync / line kernels behind their predecessors (every kernel is one wave that ends at about the same time on all SMs, so ordinary launches are the default)
     int opt_lines2 = 1;   // line pass: 1 = k_lines2 where the geometry qualifies (crt_lines2.cuh), 0 = always k_lines (A/B switch)
-    int opt_lines2_stage = 2; // k_lines2's signal staging: 2 = three 16-byte cp.async per lane and stage (measured 261 us per 296 fields),
-                              // 1 = one bulk copy (TMA) per lane and stage (286 us: 32 serial issues per warp), "tma" 0 = plain loads
+    int opt_lines2_stage = 2; // k_lines2's signal staging: 2 = three 16-byte cp.async per lane and stage,
+                              // 1 = one bulk copy (TMA) per lane and stage (32 serial issues per warp), "tma" 0 = plain loads
     int opt_host_rows = 1; // crtx_frames_host: move only the rows a field reads / writes (page-locked, 16-byte granular images)
     int opt_host_src = 0; // crtx_frames_host: read page-locked source images in place
     int opt_line_lo = 0, opt_line_hi = 1 << 30; // decoded-line window of the line pass (crtx_set_option)

@@ -3,7 +3,7 @@
 memory / spills from the ptxas log, the SASS instruction count, the mix by issue pipe and the mnemonics that
 prove the bulk-copy (TMA) and mbarrier paths are what actually got compiled.
 
-    python profiles/sass_audit.py > profiles/r1_sass_audit.txt
+    python profiles/sass_audit.py > sass_audit.txt
 """
 import collections
 import os

@@ -14,7 +14,7 @@ pkgload.load()
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def _cuda_ok():
@@ -25,10 +25,18 @@ def _cuda_ok():
         return False
 
 
-# Library variants written after the round's GPU budget was spent (checked through tests/simt/ only): their GPU
-# tests run after everything that has already been green on a B200, so that with `-x` a first-contact failure there
-# cannot hide the state of the verified variants.  Remove a name once its tests have passed on the GPU.
+# GPU tests of the variants and interfaces added last run after all the others, so that with `-x` a failure there
+# cannot hide the state of the longer-standing variants.
 NOT_YET_RUN_ON_GPU = ("template", "pv1k", "nes_p1", "nesrgb_p", "bloom", "test_gpu_wire", "test_gpu_still_cli", "test_gpu_edges", "test_gpu_fullsize", "newer_variants", "other_systems", "test_gpu_batch_api")
+
+
+@pytest.fixture(autouse=True)
+def _recorded_reference():
+    """a test that replays the reference's recorded values (support.RefEngine) starts from the first and must use all"""
+    import support
+    support.begin_reference_scope()
+    yield
+    support.end_reference_scope()
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,4 +1,4 @@
-"""Stage-by-stage GPU diagnostics (not a pytest file): run on the B200 box, prints where the CUDA
+"""Stage-by-stage GPU diagnostics (not a pytest file): run on an H100, prints where the CUDA
 pipeline first departs from the oracle.  python tests/gpu_diag.py [variant]"""
 import sys
 import traceback

@@ -209,7 +209,7 @@ static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int)
 {
     memset(p, 0, sizeof(*p));
     strcpy(p->name, "SIMT interpreter (CPU, tests only)");
-    p->major = 10;
+    p->major = 9;
     p->minor = 0;
     p->multiProcessorCount = 4; /* small grids: everything runs serially anyway */
     return cudaSuccess;

@@ -9,7 +9,10 @@
 All of them expose: set(**knobs), modulate(img, **settings), demodulate(noise) and the
 state arrays analog / inp / out / ccf / hsync / vsync / rn.
 """
+import atexit
 import ctypes as C
+import hashlib
+import json
 import os
 
 import numpy as np
@@ -175,12 +178,142 @@ class CEngine:
                     hsync=self.hsync, vsync=self.vsync, rn=self.rn)
 
 
-class RefEngine(CEngine):
+# ----------------------------------------------------------------------------------
+# the reference, recorded
+# ----------------------------------------------------------------------------------
+# A checkout without the reference sources has no oracle/_ref.  The comparisons with the reference still run there:
+# tests/golden/ref_states.json holds, per test and in call order, digests of every reference state the test compares
+# and every value it probes from a reference build.  Where oracle/_ref exists the reference itself is used, and
+#     CRT_RECORD_REF=1 python -m pytest tests/<file>.py
+# rewrites the records of the tests it runs.
+
+REF_STATES = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_states.json")
+RECORD = os.environ.get("CRT_RECORD_REF") == "1"
+_records = None
+_cursor = {}
+_recorded_now = {}
+
+
+def digest(a):
+    """64-bit sha256 prefix of an array's bytes (what the records keep of large arrays)"""
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()[:16]
+
+
+def _test_id():
+    """the running test as `<file>::<name>[params]`, independent of the directory pytest was started from"""
+    t = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0]
+    f, _, rest = t.partition("::")
+    return os.path.basename(f) + "::" + rest
+
+
+def _load_records():
+    global _records
+    if _records is None:
+        _records = json.load(open(REF_STATES)) if os.path.exists(REF_STATES) else {}
+    return _records
+
+
+def _save_records():
+    recs = dict(_load_records())
+    recs.update(_recorded_now)
+    with open(REF_STATES, "w") as f:
+        f.write("{\n" + ",\n".join("%s: %s" % (json.dumps(k), json.dumps(recs[k], separators=(",", ":")))
+                                   for k in sorted(recs)) + "\n}\n")
+
+
+def _record(value):
+    if RECORD:
+        if not _recorded_now:
+            atexit.register(_save_records)
+        tid = _test_id()
+        _recorded_now.setdefault(tid, []).append(value)  # (replaces what the file held for this test)
+    return value
+
+
+def _replay():
+    tid = _test_id()
+    recs = _load_records().get(tid)
+    k = _cursor.get(tid, 0)
+    assert recs is not None and k < len(recs), (
+        "%s: no recorded reference value #%d in %s (oracle/_ref is not built here)" % (tid, k, REF_STATES))
+    _cursor[tid] = k + 1
+    return recs[k]
+
+
+def begin_reference_scope():
+    """start of a test: its recorded reference values are consumed from the first one again (and re-recorded afresh)"""
+    tid = _test_id()
+    _cursor.pop(tid, None)
+    _recorded_now.pop(tid, None)
+
+
+def end_reference_scope():
+    """end of a test: one that replayed reference values must have compared every one of them"""
+    tid = _test_id()
+    k = _cursor.get(tid)
+    if k is not None:
+        n = len(_load_records().get(tid, []))
+        assert k == n, "%s: compared %d of the %d recorded reference values" % (tid, k, n)
+
+
+def from_reference(path, compute):
+    """compute(path) where the reference build `path` (under oracle/_ref) exists, else the value it gave when recorded.
+    The value must be JSON data: probe large outputs through digest()."""
+    if os.path.exists(path):
+        return _record(compute(path))
+    return _replay()
+
+
+STATE_KEYS = ("sync", "ccf", "analog", "inp", "out")  # a recorded state: these, in this order
+
+
+def state_digest(st):
+    return dict(sync=[int(st["hsync"]), int(st["vsync"]), int(st["rn"])], ccf=digest(np.asarray(st["ccf"], dtype=np.int64)),
+                analog=digest(st["analog"]), inp=digest(st["inp"]), out=digest(st["out"]))
+
+
+class RefState(dict):
+    """state() of the live reference: recorded when a comparison consumes it (after any masking the test applies)"""
+
+
+class RecordedState(dict):
+    """state() of the replayed reference: state_digest() of what the reference held at this point of the test"""
+
+
+class _LiveRef(CEngine):
     def __init__(self, variant, outw, outh, fmt=layout.PIX_BGRA, out=None, seed=None):
         super().__init__(ref_path(variant), variant, outw, outh, fmt, out)
         self.lib.ref_srand.argtypes = [C.c_uint]
         if seed is not None:
             self.lib.ref_srand(seed)
+
+    def state(self):
+        return RefState(super().state())
+
+
+class _ReplayRef:
+    """The reference where oracle/_ref is absent: the calls change nothing, state() hands out the recorded states in order."""
+
+    def __init__(self, variant, outw, outh, fmt=layout.PIX_BGRA, out=None, seed=None):
+        self.spec = layout.system_spec(variant)
+
+    def set(self, **kw):
+        return self
+
+    def modulate(self, img, **kw):
+        pass
+
+    def demodulate(self, noise=0):
+        pass
+
+    def state(self):
+        return RecordedState(zip(STATE_KEYS, _replay()))
+
+
+def RefEngine(variant, outw, outh, fmt=layout.PIX_BGRA, out=None, seed=None):
+    """the compiled reference (oracle/_ref/libref_<variant>.so), or its recorded states where that is not built"""
+    cls = _LiveRef if have_ref(variant) else _ReplayRef
+    return cls(variant, outw, outh, fmt, out, seed)
 
 
 class _OSys(C.Structure):
@@ -392,7 +525,16 @@ class OracleEngine:
 
 
 def assert_same_state(a, b, what=""):
-    """Bit-exact comparison of two engine states with a useful first-mismatch report."""
+    """Bit-exact comparison of two engine states with a useful first-mismatch report.  `a` may be a reference state,
+    live or recorded (see RefEngine)."""
+    if isinstance(a, RecordedState):
+        got = state_digest(b)
+        for key in STATE_KEYS:
+            assert got[key] == a[key], "%s %s: %r != %r (the reference's, recorded)" % (what, key, got[key], a[key])
+        return
+    if isinstance(a, RefState):
+        d = state_digest(a)
+        _record([d[k] for k in STATE_KEYS])
     for key in ("hsync", "vsync", "rn"):
         assert a[key] == b[key], "%s %s: %r != %r" % (what, key, a[key], b[key])
     assert np.array_equal(a["ccf"], b["ccf"]), "%s ccf: %r != %r" % (what, a["ccf"], b["ccf"])

@@ -1,5 +1,5 @@
-"""BASELINE configs[1] at the bench's full size -- a batch of 296 monitors (two per SM), 832x624 BGRA in and out,
-interlaced, blend 1, scanlines 1 -- checked through a size-independent property instead of 296 oracle runs: monitors
+"""BASELINE configs[1] at the bench's full size -- a batch of 264 monitors (two per SM of an H100), 832x624 BGRA in and out,
+interlaced, blend 1, scanlines 1 -- checked through a size-independent property instead of 264 oracle runs: monitors
 that are fed the same image, settings and noise must stay bit-identical to each other through every field (a checksum
 of checksums: one representative per group against all its members, on the device), and the representatives are
 compared with the oracle.  Also: the context's state after the run equals the oracle's for every monitor."""
@@ -11,7 +11,7 @@ from ntsc_crt_b200 import layout
 
 pytestmark = pytest.mark.gpu
 
-BATCH = 296   # bench.py's batch per GPU; tests/test_simt_kernels.py shrinks it for the CPU interpreter
+BATCH = 264   # bench.py's batch per GPU; tests/test_simt_kernels.py shrinks it for the CPU interpreter
 GROUPS = 4
 FIELDS = 4
 

@@ -3,7 +3,8 @@
 The reference has no tests or golden vectors (SURVEY.md section 4), so the pin is the
 UNMODIFIED reference compiled into oracle/_ref/libref_*.so by oracle/Makefile.  Every
 case drives both through the same call sequence and compares analog / inp / out / ccf /
-hsync / vsync / rn bit for bit after every call.
+hsync / vsync / rn bit for bit after every call.  Where oracle/_ref is not built the
+reference's side is replayed from tests/golden/ref_states.json (support.RefEngine).
 """
 import ctypes as C
 
@@ -12,9 +13,6 @@ import pytest
 
 import support as S
 from ntsc_crt_b200 import layout
-
-pytestmark = pytest.mark.skipif(not S.have_ref(), reason="oracle/_ref not built")
-
 
 def pair(variant, outw, outh, fmt=layout.PIX_BGRA, seed=1):
     ref = S.RefEngine(variant, outw, outh, fmt, seed=seed)
@@ -34,45 +32,57 @@ def check(ref, ora, what):
 def test_struct_layout_matches_reference():
     for variant in ("ntsc", "ntsc_bloom", "ntsc_conv", "ntsc_conv6", "ntsc_conv5", "ntsc_conv4", "vhs", "nes", "nes_p0", "nes_p1", "snes", "nesrgb", "nesrgb_p0", "nesrgb_p1", "template", "pv1k"):
         spec = layout.system_spec(variant)
-        lib = C.CDLL(S.ref_path(variant))
-        assert lib.ref_sizeof_crt() == C.sizeof(layout.crt_struct(spec)), variant
-        assert lib.ref_sizeof_settings() == C.sizeof(layout.settings_struct(spec)), variant
-        g = (C.c_int * 20)()
-        lib.ref_geometry(g)
-        assert list(g)[:12] == [spec.hres, spec.vres, spec.input_size, spec.top, spec.bot,
-                                spec.vper, spec.cc_samples, spec.sync_beg, spec.bw_beg, spec.cb_beg,
-                                spec.av_beg, spec.av_len], variant
-        o = (C.c_int * 19)()
-        lib.ref_crt_offsets(o)
+
+        def probe(path):
+            lib = C.CDLL(path)
+            g = (C.c_int * 20)()
+            lib.ref_geometry(g)
+            o = (C.c_int * 19)()
+            lib.ref_crt_offsets(o)
+            return [lib.ref_sizeof_crt(), lib.ref_sizeof_settings(), list(g)[:12], list(o)]
+        size_crt, size_settings, geometry, offsets = S.from_reference(S.ref_path(variant), probe)
+        assert size_crt == C.sizeof(layout.crt_struct(spec)), variant
+        assert size_settings == C.sizeof(layout.settings_struct(spec)), variant
+        assert geometry == [spec.hres, spec.vres, spec.input_size, spec.top, spec.bot,
+                            spec.vper, spec.cc_samples, spec.sync_beg, spec.bw_beg, spec.cb_beg,
+                            spec.av_beg, spec.av_len], variant
         CRT = layout.crt_struct(spec)
         names = ["analog", "inp", "outw", "outh", "out_format", "out", "hue", "brightness",
                  "contrast", "saturation", "black_point", "white_point", "scanlines", "blend",
                  "v_fac", "ccf", "hsync", "vsync", "rn"]
-        assert list(o) == [getattr(CRT, n).offset for n in names], variant
+        assert offsets == [getattr(CRT, n).offset for n in names], variant
 
 
 def test_sincos_and_bpp():
-    lib = layout.bind_crt_api(C.CDLL(S.ref_path("ntsc")), layout.system_spec("ntsc"))
+    ns = list(range(-20000, 40000, 7)) + [0, 4095, 4096, 8191, 8192, 12288, 16383, 16384]
+
+    def sincos(fn):
+        s, c, vals = C.c_int(), C.c_int(), []
+        for n in ns:
+            fn(C.byref(s), C.byref(c), n)
+            vals.append((s.value, c.value))
+        return np.array(vals, dtype=np.int64)
+
+    def probe(path):
+        lib = layout.bind_crt_api(C.CDLL(path), layout.system_spec("ntsc"))
+        return [S.digest(sincos(lib.crt_sincos14)), [lib.crt_bpp4fmt(f) for f in range(-2, 9)]]
+    want_sincos, want_bpp = S.from_reference(S.ref_path("ntsc"), probe)
     ora = S.oracle_lib()
-    s1, c1, s2, c2 = C.c_int(), C.c_int(), C.c_int(), C.c_int()
-    for n in list(range(-20000, 40000, 7)) + [0, 4095, 4096, 8191, 8192, 12288, 16383, 16384]:
-        lib.crt_sincos14(C.byref(s1), C.byref(c1), n)
-        ora.ocrt_sincos14(C.byref(s2), C.byref(c2), n)
-        assert (s1.value, c1.value) == (s2.value, c2.value), n
-    for f in range(-2, 9):
-        assert lib.crt_bpp4fmt(f) == ora.ocrt_bpp(f) == layout.bpp4fmt(f)
+    assert S.digest(sincos(ora.ocrt_sincos14)) == want_sincos
+    assert want_bpp == [ora.ocrt_bpp(f) for f in range(-2, 9)] == [layout.bpp4fmt(f) for f in range(-2, 9)]
 
 
 def test_rand_replica_matches_glibc():
-    lib = C.CDLL(S.ref_path("vhs"))
-    lib.ref_srand.argtypes = [C.c_uint]
+    """the VHS reference draws from libc's rand() (crt_core.c:344-351): the oracle's replica against libc itself"""
+    libc = C.CDLL(None)
+    libc.srand.argtypes = [C.c_uint]
     ora = S.oracle_lib()
     g = S._ORand()
     for seed in (1, 0, 42, 2**31 + 5, 0xFFFFFFFF):
-        lib.ref_srand(seed)
+        libc.srand(seed)
         ora.ocrt_rand_seed(C.byref(g), seed)
         for _ in range(2000):
-            assert lib.ref_rand() == ora.ocrt_rand_next(C.byref(g))
+            assert libc.rand() == ora.ocrt_rand_next(C.byref(g))
 
 
 def test_system_coefficients():
@@ -347,10 +357,11 @@ def test_vhs(color, aberr):
         for rec in table:
             if not rec.skip and rec.pos + ora.spec.av_len > ora.spec.input_size:
                 assert aberr, "decode window left inp[] without aberration"
-                a["out"][rec.beg:rec.end] = 0
                 b["out"][rec.beg:rec.end] = 0
-                ref.out[rec.beg:rec.end] = 0
                 ora.out[rec.beg:rec.end] = 0
+                if not isinstance(a, S.RecordedState):  # (a recorded state was recorded masked)
+                    a["out"][rec.beg:rec.end] = 0
+                    ref.out[rec.beg:rec.end] = 0
         S.assert_same_state(a, b, "vhs demod %d" % it)
 
 

@@ -46,7 +46,7 @@ def test_built_libraries_do_not_link_the_oracle():
 
 def test_the_simt_interpreter_stays_out_of_the_product():
     """tests/simt/ (the CPU interpreter that runs the kernel sources for debugging) is test infrastructure like the
-    oracle: no product loader knows its libraries, and the product libraries are real sm_100a CUDA binaries."""
+    oracle: no product loader knows its libraries, and the product libraries are real sm_90a CUDA binaries."""
     from ntsc_crt_b200 import capi
     for v in capi.VARIANTS:
         assert "simt" not in capi.lib_path(v) and os.sep + "tests" + os.sep not in capi.lib_path(v)

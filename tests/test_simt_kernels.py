@@ -2,7 +2,7 @@
 unchanged, compiled by g++ and executed one CUDA thread per fiber.  This is how kernel logic is checked in a
 container without a GPU -- block / warp synchronisation, shuffles, ballots, mbarriers and deferred bulk copies
 included -- against the same oracle and reference the `-m gpu` tests use.  It says nothing about timing, and the
-`-m gpu` tests on the B200 remain the parity proof of the real binary.
+`-m gpu` tests on the H100 remain the parity proof of the real binary.
 
 The test bodies are the ones of tests/test_gpu_*.py, re-collected here without the gpu mark; a fixture points the
 loaders at tests/simt/_build/libcrt_simt_<variant>.so and lets "device" tensors be host tensors.
@@ -115,7 +115,7 @@ def _bare(fn):
 
 
 def test_fullsize_property_on_a_small_batch(monkeypatch):
-    """tests/test_gpu_fullsize.py with 6 monitors instead of 296 (a field costs ~60 ms per monitor here)"""
+    """tests/test_gpu_fullsize.py with 6 monitors instead of 264 (a field costs ~60 ms per monitor here)"""
     monkeypatch.setattr(_fullsize, "BATCH", 6)
     monkeypatch.setattr(_fullsize, "GROUPS", 3)
     monkeypatch.setattr(_fullsize, "FIELDS", 3)

@@ -17,7 +17,7 @@ import pkgload  # noqa: E402
 pkgload.load()
 from ntsc_crt_b200 import capi, layout  # noqa: E402
 
-B, W, H = 296, 832, 624
+B, W, H = 264, 832, 624
 dev = torch.device("cuda", 0)
 gen = torch.Generator(device="cpu").manual_seed(1234)
 src = torch.randint(0, 256, (B, H, W, 4), dtype=torch.uint8, generator=gen).to(dev)

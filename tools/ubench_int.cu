@@ -1,6 +1,6 @@
 // ubench_int.cu -- issue-rate micro-benchmark of the integer instructions the line kernels are made of
 // (IMAD, IMAD.HI with 64-bit addend, SHF, LEA.HI.SX32, IADD3) on one SM sub-partition set.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench_int ubench_int.cu ; run: ./ubench_int
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench_int ubench_int.cu ; run: ./ubench_int
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,6 +1,6 @@
 // ubench_pcie.cu -- how fast can SM-issued loads / stores move rows between page-locked host memory and HBM, compared with
 // the copy engines?  (crtx_frames_host moves irregularly spaced rows with copy kernels, csrc/crtx.cu k_rows_gather /
-// k_rows_scatter.)   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench_pcie ubench_pcie.cu ; ./ubench_pcie
+// k_rows_scatter.)   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench_pcie ubench_pcie.cu ; ./ubench_pcie
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -73,7 +73,7 @@ int main()
         printf("copy engine   D2H whole            %7.2f GB/s\n", total / ms / 1e6);
     }
     for (int depth : { 4, 8, 13 })
-        for (int grid : { 148, 148 * 4, 148 * 8 }) {
+        for (int grid : { 132, 132 * 4, 132 * 8 }) {
             Job g = { h_a, d_a, rows, n16, n16, n16, grid, depth, 0 };
             float ms = timed(s1, 5, run_kernel, &g);
             Job s = { d_a, h_b, rows, n16, n16, n16, grid, depth, 0 };
@@ -82,8 +82,8 @@ int main()
                    total / ms / 1e6, total / ms2 / 1e6);
         }
     { // every third row only (what a field touches), both directions at once on two streams
-        Job g = { h_a, d_a, rows / 3, n16, 3 * n16, n16, 148 * 8, 8, 0 };
-        Job s = { d_b, h_b, rows / 3, n16, n16, 3 * n16, 148 * 8, 8, 0 };
+        Job g = { h_a, d_a, rows / 3, n16, 3 * n16, n16, 132 * 8, 8, 0 };
+        Job s = { d_b, h_b, rows / 3, n16, n16, 3 * n16, 132 * 8, 8, 0 };
         cudaEvent_t a, b, c;
         cudaEventCreate(&a); cudaEventCreate(&b); cudaEventCreate(&c);
         cudaDeviceSynchronize();
@@ -118,7 +118,7 @@ int main()
         cudaEventCreate(&a); cudaEventCreate(&b); cudaEventCreate(&c);
         const int starts[5] = { 0, 2, 5, 7, 10 }, widths[5] = { 1, 2, 1, 2, 2 }; // rows written per 13-row period (scanlines 1)
         for (int mode = 0; mode < 3; mode++) {
-            Job g = { h_a, d_a, frames * 236, n16, 0, n16, 148 * 8, 8, 0 };
+            Job g = { h_a, d_a, frames * 236, n16, 0, n16, 132 * 8, 8, 0 };
             cudaDeviceSynchronize();
             cudaEventRecord(a, s1);
             cudaStreamWaitEvent(s2, a, 0);
@@ -151,7 +151,7 @@ int main()
         cudaEventCreate(&a); cudaEventCreate(&b); cudaEventCreate(&c);
         const int starts[5] = { 0, 2, 5, 7, 10 };
         for (int mode = 0; mode < 3; mode++) {
-            Job sc = { d_b, h_b, frames * 384, n16, n16, n16 * 624 / 384, 148 * 8, 8, 0 };
+            Job sc = { d_b, h_b, frames * 384, n16, n16, n16 * 624 / 384, 132 * 8, 8, 0 };
             cudaDeviceSynchronize();
             cudaEventRecord(a, s1);
             cudaStreamWaitEvent(s2, a, 0);

@@ -1,8 +1,8 @@
-// ubench_pipes.cu -- which pipe the integer instructions of the kernels use on sm_100a and at what rate: every case is a loop of
+// ubench_pipes.cu -- which pipe the integer instructions of the kernels use on sm_90a and at what rate: every case is a loop of
 // 8 independent chains per thread, 16 warps on one SM (4 per scheduler); "A + B" cases interleave two instructions -- if the
 // pair costs max(A, B) they issue to different pipes, if it costs A + B they share one.  The instruction actually generated
-// is whatever cuobjdump -sass shows for the case (checked in profiles/r2_ubench_pipes.txt).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench_pipes ubench_pipes.cu ; run: ./ubench_pipes
+// is whatever cuobjdump -sass shows for the case.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench_pipes ubench_pipes.cu ; run: ./ubench_pipes
 #include <cstdio>
 #include <cuda_runtime.h>
 
