@@ -376,8 +376,9 @@ __global__ void __launch_bounds__(256) k_mod_picture_rgb(const SrcCfg *__restric
 // data movement: a lane owns a picture line for the whole pass (the IIRs are serial along it), and
 // the stretch of its source row that a 32-sample chunk maps to is brought into shared memory by a
 // 1-D TMA bulk copy (one per lane, double buffered), so the serial loop reads pixels at
-// shared-memory latency and no transposition of the input is needed.  Finished samples are packed
-// 4 to a word and written back with coalesced 2-byte stores.
+// shared-memory latency and no transposition of the input is needed.  Which source pixel a sample
+// reads is tabulated once per CTA.  Finished samples are packed 4 to a word and written back in
+// windows aligned to 32-byte sectors (put, below).
 // Usable when the chunk's source span fits a stage row; other monitors return at once and are
 // handled by k_mod_picture_rgb (gather variant), which in turn skips the ones done here.
 // The source image must be readable up to the next 16-byte boundary past its last pixel
@@ -390,9 +391,12 @@ constexpr int kModSSpan = 192;                     // largest staged span the ke
 // banks (16-way); 176 B (44 words) spreads them over 8 (4-way,
 // the best a 16-byte granular pitch can do).  176 is also exactly the largest copy an accepted span needs.
 constexpr int kModSRow = 176;
-constexpr int kModSOutPitch = kModSChunk / 4 + 1;  // words
-constexpr int kModSWarpSmem = 2 * 32 * kModSRow + 32 * kModSOutPitch * 4 + 32 * 4;
-constexpr int kModSSmem = 8 * kModSWarpSmem + 8 * 2 * 8;
+constexpr int kModSOutPitch = 2 * kModSChunk / 4 + 1;  // words: a ring of two chunks' output per line
+constexpr int kModSWarpSmem = 2 * 32 * kModSRow + 32 * kModSOutPitch * 4;
+// Behind the eight warps' areas: their mbarriers, then the monitor's column table -- the byte offset of sample x's source
+// pixel from the first pixel of x's chunk, for whole chunks -- and each chunk's first and last source column.
+constexpr int kModSCols = (kDestW + kModSChunk - 1) / kModSChunk * kModSChunk;
+constexpr int kModSSmem = 8 * kModSWarpSmem + 8 * 2 * 8 + kModSCols * 4 + kModSCols / kModSChunk * 8;
 
 __host__ __device__ __forceinline__ bool mod_staged_ok(const SrcCfg &s, int destw)
 {
@@ -479,8 +483,9 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
 
     unsigned char *stage = smem_raw + warp * kModSWarpSmem;
     unsigned *obuf = reinterpret_cast<unsigned *>(stage + 2 * 32 * kModSRow);
-    int *coltab = reinterpret_cast<int *>(obuf + 32 * kModSOutPitch);
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + 8 * kModSWarpSmem) + 2 * warp;
+    unsigned *coltab = reinterpret_cast<unsigned *>(smem_raw + 8 * kModSWarpSmem + 8 * 2 * 8);
+    uint2 *spans = reinterpret_cast<uint2 *>(coltab + kModSCols);
 
     constexpr int bpp = (FMT <= 1) ? 3 : 4;
     constexpr int rp = (FMT == 0 || FMT == 3) ? 0 : (FMT == 2) ? 1 : (FMT == 4) ? 3 : 2; // crt_core.h:62-67
@@ -492,17 +497,25 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
         desth = min(s.h, kDestH);
     }
     if (desth <= 0 || s.h <= 0) return;
+    const int nchunks = (destw + kModSChunk - 1) / kModSChunk;
+    // sample x reads source column (x * w) / destw (crt_ntsc.c:272), which depends on the monitor alone: tabulated once here
+    // as a byte offset from the first pixel of x's chunk (samples past destw repeat the last column), with every chunk's
+    // span of columns, instead of a division per lane per chunk in every warp
+    for (int x = (int) threadIdx.x; x < nchunks * kModSChunk; x += (int) blockDim.x) {
+        const unsigned col = (unsigned) min(x, destw - 1) * (unsigned) s.w / (unsigned) destw;
+        const unsigned f0 = (unsigned) (x & ~(kModSChunk - 1)) * (unsigned) s.w / (unsigned) destw;
+        coltab[x] = (col - f0) * bpp;
+        if ((x & (kModSChunk - 1)) == kModSChunk - 1) spans[x / kModSChunk] = make_uint2(f0, col);
+    }
     // five carrier phases (PV-1000): the phase of a sample is not a compile-time constant of the 4-sample inner step, so the
     // tables live in shared memory, [I | Q][colour row][phase], as in the gather kernel
     __shared__ int mtab[2][kVper][kCc];
-    if (kCc == 5) {
-        if (threadIdx.x < kCc * kVper) {
-            int b;
-            enc_tables(s, (int) threadIdx.x / kCc, (int) threadIdx.x % kCc, b, mtab[0][threadIdx.x / kCc][threadIdx.x % kCc],
-                       mtab[1][threadIdx.x / kCc][threadIdx.x % kCc]);
-        }
-        __syncthreads(); // (every return above is block-uniform)
+    if (kCc == 5 && threadIdx.x < kCc * kVper) {
+        int b;
+        enc_tables(s, (int) threadIdx.x / kCc, (int) threadIdx.x % kCc, b, mtab[0][threadIdx.x / kCc][threadIdx.x % kCc],
+                   mtab[1][threadIdx.x / kCc][threadIdx.x % kCc]);
     }
+    __syncthreads(); // (every return above is block-uniform)
     const int y0 = warp * 32;
     if (y0 >= desth) return;
     const int nlines = min(32, desth - y0);
@@ -546,28 +559,36 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
     if (row >= s.h) row = s.h - 1;
     if (s.compact) row = y; // crtx_frames_host staged exactly those rows, in line order (k_rows_gather)
     const unsigned char *rowp = data + (size_t) row * s.w * bpp;
-    const int nchunks = (destw + kModSChunk - 1) / kModSChunk;
+    // cp.async staging copies the warp's spans four lanes to a row, eight rows at a time: the source rows of lines
+    // 8j + lane / 4, j = 0 .. 3
+    unsigned long long rowoffs[4];
+#pragma unroll
+    for (int j = 0; j < 4; j++) rowoffs[j] = __shfl_sync(0xffffffffu, (unsigned long long) row * s.w * bpp, j * 8 + (lane >> 2));
 
-    // chunk c covers samples [32c, 32c + 32): lane l maps sample 32c + l to source column
-    // (x * w) / destw (crt_ntsc.c:272) -- one 32-bit division per lane per chunk, computed one chunk
-    // ahead; the chunk's span f0..f1 is staged from the 16-byte aligned address at or below pixel f0
-    auto colof = [&](int c) {
-        const unsigned x = (unsigned) min(c * kModSChunk + lane, destw - 1);
-        return (int) (x * (unsigned) s.w / (unsigned) destw);
-    };
-    auto issue = [&](int c, int col) {
-        const int nxc = min(kModSChunk, destw - c * kModSChunk);
-        const int f0 = __shfl_sync(0xffffffffu, col, 0), f1 = __shfl_sync(0xffffffffu, col, nxc - 1);
-        const int bytes = (f1 - f0 + 1) * bpp;
-        const unsigned char *p = rowp + (size_t) f0 * bpp;
+    // chunk c covers samples [32c, 32c + 32); its span of source columns f0..f1 is staged from the 16-byte aligned address
+    // at or below pixel f0.  Returns the offset of pixel f0 from that address.
+    auto issue = [&](int c) {
+        const uint2 sp = spans[c];
+        const int bytes = (int) (sp.y - sp.x + 1) * bpp;
+        const unsigned char *p = rowp + (size_t) sp.x * bpp;
         const int a = (int) (reinterpret_cast<uintptr_t>(p) & 15);
         const unsigned copy = (unsigned) ((a + bytes + 15) & ~15);
         unsigned char *dst = stage + (c & 1) * 32 * kModSRow + lane * kModSRow;
-        if (use_tma == 2) { // per-lane 16-byte asynchronous copies, one group per chunk
-            if (active) {
+        if (use_tma == 2) {
+            // 16-byte asynchronous copies, one group per chunk.  Four neighbouring lanes fetch neighbouring 16-byte pieces
+            // of one row, so a copy instruction touches eight rows' spans instead of 32.
 #pragma unroll
-                for (unsigned q = 0; q < kModSRow / 16; q++)
-                    if (q * 16 < copy) cp_async_16(dst + q * 16, p - a + q * 16);
+            for (int j = 0; j < 4; j++) {
+                const int r = j * 8 + (lane >> 2);
+                const unsigned char *pr = data + rowoffs[j] + (size_t) sp.x * bpp;
+                const int ar = (int) (reinterpret_cast<uintptr_t>(pr) & 15);
+                const unsigned copyr = (unsigned) ((ar + bytes + 15) & ~15);
+                unsigned char *dr = stage + (c & 1) * 32 * kModSRow + r * kModSRow;
+#pragma unroll
+                for (unsigned k = 0; k < (kModSRow / 16 + 3) / 4; k++) {
+                    const unsigned q = k * 4 + (lane & 3);
+                    if (r < nlines && q * 16 < copyr) cp_async_16(dr + q * 16, pr - ar + q * 16);
+                }
             }
             cp_async_commit();
         } else if (use_tma) {
@@ -582,6 +603,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
             for (unsigned q = 0; q < copy / 16; q++)
                 reinterpret_cast<uint4 *>(dst)[q] = __ldg(reinterpret_cast<const uint4 *>(p - a) + q);
         }
+        return a;
     };
 
     // the rows of the RGB -> YIQ matrix (crt_ntsc.c:308-310) for 4-byte pixels, see YiqDot
@@ -596,39 +618,65 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
             dot_q.init(zero);
         }
     }
+    // Stores.  A line's finished bytes go out in windows that end on a 32-byte boundary of analog[]: eight lanes write one
+    // line's window as aligned words, four lines per instruction, so every sector but the first and last of a line is
+    // written whole, once.  (Partly written sectors cost the memory system a read of the sector; 2-byte stores per chunk
+    // left two of them per line and chunk.)  put(c) writes the window [e - 32, e) whose end e lies in (32c, 32c + 32],
+    // cut to [0, destw): after chunk c all of it is in the line's 64-byte ring, chunk c - 1 in one half, chunk c in the other.
+    auto put = [&](int c) {
+        const int t = lane & 7;
+#pragma unroll
+        for (int i = 0; i < 32 / 4; i++) {
+            const int L = 4 * i + (lane >> 3);
+            if (L >= nlines) continue;
+            signed char *ln = analog + (y0 + L + yo) * kHres + xo;
+            const int e0 = (int) ((0u - (unsigned) reinterpret_cast<uintptr_t>(ln)) & 31u);
+            const int x = c * kModSChunk + (e0 ? e0 : 32) - 32 + 4 * t; // ln + x is a multiple of 4
+            if (x >= destw || x + 4 <= 0) continue;
+            const unsigned *ring = obuf + L * kModSOutPitch;
+            const int pos = x & (2 * kModSChunk - 1);
+            const unsigned long long two = ring[pos >> 2] | ((unsigned long long) ring[((pos >> 2) + 1) & (2 * kModSChunk / 4 - 1)] << 32);
+            const unsigned v = (unsigned) (two >> (8 * (pos & 3)));
+            if (x >= 0 && x + 4 <= destw) {
+                *reinterpret_cast<unsigned *>(ln + x) = v;
+            } else {
+                for (int b = 0; b < 4; b++)
+                    if (x + b >= 0 && x + b < destw) ln[x + b] = (signed char) (v >> (8 * b));
+            }
+        }
+    };
     int hy = 0, hi = 0, hq = 0;
-    int col_cur = colof(0);
-    issue(0, col_cur);
+    int a_cur = issue(0);
 #pragma unroll 1
     for (int c = 0; c < nchunks; c++) {
-        int col_nxt = 0;
-        if (c + 1 < nchunks) {
-            col_nxt = colof(c + 1);
-            issue(c + 1, col_nxt);
-        }
-        const int f0 = __shfl_sync(0xffffffffu, col_cur, 0);
+        const int a_nxt = (c + 1 < nchunks) ? issue(c + 1) : 0;
         const int c0 = c * kModSChunk;
-        const int nx = min(kModSChunk, destw - c0);
-        coltab[lane] = (col_cur - f0) * bpp; // byte offset of sample x's pixel from the chunk's first pixel
-        col_cur = col_nxt;
-        if (use_tma == 2) { // this lane's own row: everything but the chunk just requested has landed
+        if (use_tma == 2) { // every lane's copies but those of the chunk just requested have landed (visible to all after the __syncwarp)
             if (c + 1 < nchunks) cp_async_wait<1>();
             else cp_async_wait<0>();
         } else if (use_tma) {
             mbar_wait(&bars[c & 1], (c >> 1) & 1);
         }
         __syncwarp();
-        const unsigned char *srow = stage + (c & 1) * 32 * kModSRow + lane * kModSRow
-                                  + (int) (reinterpret_cast<uintptr_t>(rowp + (size_t) f0 * bpp) & 15);
+        const unsigned char *srow = stage + (c & 1) * 32 * kModSRow + lane * kModSRow + a_cur;
+        a_cur = a_nxt;
         int p5 = c0 % 5; // carrier phase of the chunk's first sample (five-phase systems)
-#pragma unroll 1
-        for (int x4 = 0; x4 < nx; x4 += 4) { // kModSChunk is a multiple of 4: coltab[x4 .. x4 + 3] exist
-            unsigned packed = 0;
+        // The whole chunk, straight-line: no sample's fetch or RGB -> YIQ waits for the IIR chains of the samples before it,
+        // so the compiler overlaps them with those chains.  The last chunk runs whole as well: the samples past destw read
+        // the last column (the table repeats it), move nothing but this line's IIR state after its last stored sample, and
+        // are not stored.
+        const uint4 *offs = reinterpret_cast<const uint4 *>(coltab + c0);
+        unsigned packed[kModSChunk / 4];
+#pragma unroll
+        for (int g = 0; g < kModSChunk / 4; g++) {
+            const uint4 o4 = offs[g];
+            const unsigned off4[4] = {o4.x, o4.y, o4.z, o4.w};
+            unsigned word = 0;
             int rr[4], gg[4], bb[4];
             unsigned pix[4];
 #pragma unroll
-            for (int k = 0; k < 4; k++) { // all four pixel fetches first, then the dependent arithmetic
-                const int off = coltab[x4 + k];
+            for (int k = 0; k < 4; k++) {
+                const int off = (int) off4[k];
                 if (bpp == 4) {
                     pix[k] = *reinterpret_cast<const unsigned *>(srow + off);
                 } else {
@@ -662,53 +710,23 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
                     if (kCc == 5) { // (x + xo) % 5 == x % 5: xo is a multiple of 5; p5 walks 0 .. 4 along the line
                         sum += (wmul(hi, mtab[0][crow][p5]) >> 4) + (wmul(hq, mtab[1][crow][p5]) >> 4);
                         p5 = (p5 == 4) ? 0 : p5 + 1;
-                    } else { // (x + xo) & 3 == k: xo, c0 and x4 are multiples of 4
+                    } else { // (x + xo) & 3 == k: xo and c0 are multiples of 4
                         sum += (wmul(hi, mI[k]) >> 4) + (wmul(hq, mQ[k]) >> 4);
                     }
                 }
                 int ire = ire0 + (wmul(sum, white) >> 10);
                 ire = __vimin_s32_relu(ire, 110); // clamp to 0..110 in one instruction
-                packed |= (unsigned) ire << (8 * k);
+                word |= (unsigned) ire << (8 * k);
             }
-            obuf[lane * kModSOutPitch + (x4 >> 2)] = packed;
+            packed[g] = word;
         }
+#pragma unroll
+        for (int g = 0; g < kModSChunk / 4; g++) obuf[lane * kModSOutPitch + (c & 1) * (kModSChunk / 4) + g] = packed[g];
         __syncwarp();
-        // coalesced stores: 16 lanes x 2 bytes per line, two lines per pass
-        {
-            const int j = lane & 15;
-            const unsigned short *ob = reinterpret_cast<const unsigned short *>(obuf) + (lane >> 4) * (2 * kModSOutPitch) + j;
-            signed char *dst = analog + (c0 + xo) + (y0 + (lane >> 4) + yo) * kHres + 2 * j;
-            // the pair is 2-byte aligned when xo is even: always with four carrier phases (xo is a multiple of 4 and CRT_HRES is
-            // even), not with the PV-1000's five (xo is a multiple of 5); dst moves by whole pairs of lines, so its parity stays
-            if (kCc == 5 && (reinterpret_cast<uintptr_t>(dst) & 1)) {
-                for (int l2 = 0; l2 < nlines; l2 += 2) {
-                    if (l2 + (lane >> 4) < nlines) {
-                        const unsigned short two = ob[l2 * (2 * kModSOutPitch)];
-                        if (2 * j < nx) dst[0] = (signed char) (two & 0xff);
-                        if (2 * j + 1 < nx) dst[1] = (signed char) (two >> 8);
-                    }
-                    dst += 2 * kHres;
-                }
-            } else if (nx == kModSChunk) { // full chunk: no edge tests
-#pragma unroll 4
-                for (int l2 = 0; l2 + 1 < nlines; l2 += 2) {
-                    *reinterpret_cast<unsigned short *>(dst) = ob[l2 * (2 * kModSOutPitch)];
-                    dst += 2 * kHres;
-                }
-                if ((nlines & 1) && lane < 16) *reinterpret_cast<unsigned short *>(dst) = ob[(nlines - 1) * (2 * kModSOutPitch)];
-            } else {
-                for (int l2 = 0; l2 < nlines; l2 += 2) {
-                    if (l2 + (lane >> 4) < nlines) {
-                        const unsigned short two = ob[l2 * (2 * kModSOutPitch)];
-                        if (2 * j + 1 < nx) *reinterpret_cast<unsigned short *>(dst) = two;
-                        else if (2 * j < nx) *dst = (signed char) (two & 0xff);
-                    }
-                    dst += 2 * kHres;
-                }
-            }
-        }
+        put(c);
         __syncwarp();
     }
+    put(nchunks); // the rest of every line
     phase_mark(2, 14);
     phase_mark(2, 12, 7 * 32);
 }
