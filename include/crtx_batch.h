@@ -150,6 +150,13 @@ long crtx_launch_count(crtx_ctx *ctx); /* kernels launched through this context 
 long crtx_lines2_count(crtx_ctx *ctx); /* of those, line passes taken by k_lines2 (two monitors per CTA, tabulated resampler: the
                                          * stock IIR decoder on 4-byte pixels, 16-byte aligned images, outw a multiple of 4 in about
                                          * [528, 1312]); every other geometry runs k_lines.  For tests and A/B runs (option "lines2"). */
+/* which code paths monitors [first, first + count) took: paths[i] has CRTX_PATH_GENERIC_EQ set when the last demodulate's sync
+ * pass put monitor first + i on the wrap-exact equaliser (its carrier or brightness is outside the fast equaliser's exact range,
+ * or option "generic_eq" is on), and CRTX_PATH_STAGED_MOD when the last modulate encoded its picture with the staged encoder
+ * (the source span of a 32-sample chunk fits a stage row) rather than the gather encoder.  Synchronises `stream`. */
+#define CRTX_PATH_GENERIC_EQ 1
+#define CRTX_PATH_STAGED_MOD 2
+int crtx_get_paths(crtx_ctx *ctx, int first, int count, int *paths, void *stream);
 /* options: "tma", "generic_eq", "timing", "mod_staged", "fused_noise", "mod_bulk", "lines2", "host_rows", "pdl" (0/1 switches; "pdl" 1 launches the
  * picture, sync and line kernels as programmatic dependents of their predecessors, default 0), "lines2_stage" (how k_lines2 stages
  * the signal windows: 2 = cp.async, the default; 1 = one bulk copy per lane), "host_src" (1:

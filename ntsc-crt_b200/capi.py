@@ -59,8 +59,8 @@ CRTX_EXPORTS = ("crtx_system", "crtx_chroma_pattern", "crtx_hres", "crtx_input_s
                 "crtx_cc_vper", "crtx_create", "crtx_destroy", "crtx_set_monitors", "crtx_set_state",
                 "crtx_get_state", "crtx_seed", "crtx_analog", "crtx_inp", "crtx_read_signal",
                 "crtx_write_signal", "crtx_modulate",
-                "crtx_demodulate", "crtx_frames_host", "crtx_get_lines", "crtx_launch_count", "crtx_lines2_count",
-                "crtx_set_option", "crtx_get_timing", "crtx_last_error")
+                "crtx_demodulate", "crtx_frames_host", "crtx_get_lines", "crtx_get_paths", "crtx_launch_count",
+                "crtx_lines2_count", "crtx_set_option", "crtx_get_timing", "crtx_last_error")
 
 _libs = {}
 
@@ -94,6 +94,7 @@ def load(variant):
     lib.crtx_demodulate.argtypes = [vp, ip, ip, vp]
     lib.crtx_frames_host.argtypes = [vp, ip, ip, C.POINTER(Source), C.POINTER(vp), vp]
     lib.crtx_get_lines.argtypes = [vp, ip, C.POINTER(Line), vp]
+    lib.crtx_get_paths.argtypes = [vp, ip, ip, C.POINTER(C.c_int), vp]
     lib.crtx_launch_count.argtypes = [vp]
     lib.crtx_launch_count.restype = C.c_long
     lib.crtx_lines2_count.argtypes = [vp]
@@ -205,6 +206,16 @@ class Batch:
         t = (Line * self.spec.lines)()
         self._check(self.lib.crtx_get_lines(self._ctx, i, t, stream))
         return t
+
+    PATH_GENERIC_EQ = 1  # CRTX_PATH_GENERIC_EQ: the last demodulate decoded the monitor with the wrap-exact equaliser
+    PATH_STAGED_MOD = 2  # CRTX_PATH_STAGED_MOD: the last modulate encoded its picture with the staged encoder
+
+    def paths(self, first=0, count=None, stream=0):
+        """crtx_get_paths: per monitor, the PATH_* bits of the code paths its last modulate and demodulate took"""
+        count = self.n - first if count is None else count
+        out = (C.c_int * count)()
+        self._check(self.lib.crtx_get_paths(self._ctx, first, count, out, stream))
+        return list(out)
 
     def analog_ptr(self, i):
         return self.lib.crtx_analog(self._ctx, i)

@@ -38,7 +38,7 @@ __device__ __forceinline__ int pole(int f, int in, int rnd)
 // One eqf() step (crt_core.c:205-233).
 // FAST is exact when every Q16 gain of 65536 is an identity and no product wraps, i.e. every band
 // stays below 32768 in magnitude.  k_sync guarantees that per monitor from max|s| * |wave| >> 9 <= 16382
-// (chroma inputs <= 16383; a one-pole stage with 0 < c <= 65536 never leaves the range of its inputs,
+// (chroma inputs <= 16383; |s| <= 127 inside inp[], 128 for a line whose window reaches the struct tail behind it; a one-pole stage with 0 < c <= 65536 never leaves the range of its inputs,
 // so |fH3 - fL3| < 32768) and |bright| <= 4096 (luma; the hf = 79824 cascade overshoots by at most 1.558^4).  Then for I and Q
 // r0 + r1 == fH[3] exactly -- their low cascades cancel and are not evaluated at all -- and Y's
 // middle gain 8192 is an arithmetic shift by 3.

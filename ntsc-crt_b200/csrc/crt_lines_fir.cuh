@@ -45,7 +45,8 @@ static_assert(kFirSeg % 32 == 0, "whole warp steps per segment");
 // always finds sample s + 1 in the slot after sample s.  FAST keeps 16-bit entries, which the resampler
 // reads with sign-extending loads; they fit because the kernels have unit DC gain and k_sync only leaves
 // a monitor on the FAST path when |bright| <= 4096 (|Y| <= 127 + 4096 before the x16 the pixel pass
-// applies) and every chroma input (s * wave) >> 9 is within +-16383 (|I|, |Q| <= 2048 after the >> 3).
+// applies) and every chroma input (s * wave) >> 9 is within +-16383 (|I|, |Q| <= 2048 after the >> 3), counting |s| = 128 for a
+// line whose window reaches the struct tail behind inp[] (crt_sync.cuh).
 template <bool FAST> struct FirRow {
     using Elem = typename std::conditional<FAST, short, int>::type;
     static constexpr int kSlots = 1 + kFirSamples + kFirSamples / 8;

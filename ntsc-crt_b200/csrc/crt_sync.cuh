@@ -642,13 +642,17 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
                 for (int i = 0; i < 5; i++) wmax = max(wmax, max(llabs((long long) wi[i]), llabs((long long) wq[i])));
             }
             // The fast equaliser path of k_lines is exact while every chroma input (s * wave) >> 9 stays
-            // within +-16383 (crt_lines.cuh).  |s| <= 127 always (the clamp of crt_core.c:363-364).  With the stock
-            // saturation that bound already passes and nothing more is needed; only a line whose carrier is large enough
-            // to fail it needs the real maximum of its two signal lines.  Measuring that costs about as much as the copy itself,
-            // so it is done only for monitors that needed it the last time (MonState::track_max: the NES and NES-RGB
-            // systems at their stock saturation, nothing else at stock settings), inside the copy that runs beside the
+            // within +-16383 (crt_lines.cuh).  The line reads samples [pos, pos + AV_LEN).  Inside inp[] |s| <= 127 (the
+            // clamp of crt_core.c:363-364); a window that runs past the end of inp[] (the PV-1000's last signal line, in
+            // ordinary operation) also reads the struct tail behind it (k_struct_tail), bytes that are neither clamped nor
+            // measured below, and -128 whenever a byte of outw or outh is 0x80 (outw = 640): such a line counts |s| = 128.
+            // With the stock saturation that bound already passes and nothing more is needed; only a line whose carrier is
+            // large enough to fail it needs the real maximum of its two signal lines.  Measuring that costs about as much as
+            // the copy itself, so it is done only for monitors that needed it the last time (MonState::track_max: the NES and
+            // NES-RGB systems at their stock saturation, nothing else at stock settings), inside the copy that runs beside the
             // burst-lock chain; the first pass of such a monitor scans the two lines here instead, one thread per line, slowly.
-            int smax = 127;
+            const int stail = (rec.pos + kAvLen > kInputSize) ? 128 : 0;
+            int smax = max(127, stail);
             if (FUSED && ((smax * wmax) >> 9) + 1 > 16383) {
                 sh.need_max = 1; // (the next pass of this monitor measures while it copies)
                 if (track) {
@@ -659,6 +663,7 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
                     for (int i = lo; i < hi; i++) mx = max(mx, abs((int) inp_w[i]));
                     smax = mx;
                 }
+                smax = max(smax, stail);
             }
             if (((smax * wmax) >> 9) + 1 > 16383) sh.generic = 1;
         }

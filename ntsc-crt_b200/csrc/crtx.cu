@@ -375,8 +375,11 @@ int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cuda
     // The gather kernel only runs for sources the staged one cannot take (their span does not fit a stage row), or for all of
     // them when staging is off: the host can tell (mod_takes is a pure function of the settings), so the usual call saves a launch.
     bool gather = !staged;
-    for (int i = 0; i < count; i++)
-        if (bpp_of(src[i].format) != 0 && staged && !mod_takes<true>(src[i])) gather = true;
+    for (int i = 0; i < count; i++) {
+        const bool takes = bpp_of(src[i].format) != 0 && staged && mod_takes<true>(src[i]);
+        if (bpp_of(src[i].format) != 0 && staged && !takes) gather = true;
+        ctx->h_mod_staged[first + i] = takes ? 1 : 0;
+    }
     {
         LaunchTimer lt(ctx, stream, 0);
         k_mod_skeleton_rgb<<<count, 256, 0, stream>>>(ctx->d_src + first, ctx->d_state, ctx->d_analog, first);
@@ -767,6 +770,7 @@ int crtx_create(crtx_ctx **out, int n)
     ctx->sm_count = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 132;
     ctx->h_cfg.assign(n, MonCfg());
     memset(ctx->h_cfg.data(), 0, sizeof(MonCfg) * n);
+    ctx->h_mod_staged.assign(n, 0);
     ctx->cfg_dirty_lo = 0;
     ctx->cfg_dirty_hi = n;
     ctx->tail_dirty_lo = 0;
@@ -1142,6 +1146,20 @@ int crtx_get_lines(crtx_ctx *ctx, int i, crtx_line *table, void *stream)
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CUDA_TRY(cudaMemcpyAsync(table, ctx->d_lines + (size_t) i * kLines, sizeof(LineRec) * kLines, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+
+int crtx_get_paths(crtx_ctx *ctx, int first, int count, int *paths, void *stream)
+{
+    if (check_range(ctx, first, count)) return 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    std::vector<MonState> tmp(count);
+    if (count > 0) {
+        CUDA_TRY(cudaMemcpyAsync(tmp.data(), ctx->d_state + first, sizeof(MonState) * count, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+    }
+    for (int i = 0; i < count; i++)
+        paths[i] = (tmp[i].generic ? CRTX_PATH_GENERIC_EQ : 0) | (ctx->h_mod_staged[first + i] ? CRTX_PATH_STAGED_MOD : 0);
     return 0;
 }
 

@@ -36,6 +36,7 @@ struct crtx_ctx {
     unsigned char *d_src_img = nullptr; // crtx_frames_host staging, src_slot bytes per monitor
     size_t src_slot = 0;
     std::vector<crt::MonCfg> h_cfg;
+    std::vector<unsigned char> h_mod_staged; // per monitor: the last modulate encoded its picture with k_mod_picture_rgb_staged (crtx_get_paths)
     std::vector<crt::SrcCfg> scratch_src;
     int cfg_dirty_lo = 0, cfg_dirty_hi = 0;
     int tail_dirty_lo = 0, tail_dirty_hi = 0; // monitors whose output geometry changed: k_struct_tail rewrites the bytes behind their signals

@@ -25,6 +25,7 @@ import test_gpu_dropin_cli as _cli  # noqa: E402
 import test_gpu_edges as _edges  # noqa: E402
 import test_gpu_fullsize as _fullsize  # noqa: E402
 import test_gpu_fuzz as _fuzz  # noqa: E402
+import test_gpu_guard_edges as _guard  # noqa: E402
 import test_gpu_lines2 as _lines2  # noqa: E402
 import test_gpu_lineshard as _lineshard  # noqa: E402
 import test_gpu_parity as _parity  # noqa: E402
@@ -101,6 +102,7 @@ _adopt(_pv1k, "pv1k")
 _adopt(_wire, "wire")
 _adopt(_bloom, "bloom")
 _adopt(_api, "api")
+_adopt(_guard, "guard")
 test_cli_unmodified_cli_driver_is_byte_identical = _cli.test_unmodified_cli_driver_is_byte_identical
 _adopt(_still, "still")
 test_vconv_unmodified_video_convert_runs_against_the_library = _vconv.test_unmodified_video_convert_runs_against_the_library
