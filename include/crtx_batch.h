@@ -157,9 +157,7 @@ long crtx_lines2_count(crtx_ctx *ctx); /* of those, line passes taken by k_lines
 #define CRTX_PATH_GENERIC_EQ 1
 #define CRTX_PATH_STAGED_MOD 2
 int crtx_get_paths(crtx_ctx *ctx, int first, int count, int *paths, void *stream);
-/* options: "tma", "generic_eq", "timing", "mod_staged", "fused_noise", "mod_bulk", "lines2", "host_rows", "pdl" (0/1 switches; "pdl" 1 launches the
- * picture, sync and line kernels as programmatic dependents of their predecessors, default 0), "lines2_stage" (how k_lines2 stages
- * the signal windows: 2 = cp.async, the default; 1 = one bulk copy per lane), "host_src" (1:
+/* options: "generic_eq", "timing", "mod_staged", "lines2", "host_rows" (0/1 switches), "host_src" (1:
  * crtx_frames_host lets the encoder read page-locked source images in place instead of copying them), and
  * "line_lo" / "line_hi": crtx_demodulate's line pass only decodes scanlines [line_lo, line_hi) of every
  * field (sync search and noise still cover the whole field).  This is the scanline-block partition of

@@ -4,8 +4,8 @@
 //   k_mod_skeleton_rgb  sync / blanking / burst skeleton of all 262 lines  crt_ntsc.c:205-252, 325-329
 //   k_mod_picture_rgb   RGB->YIQ, 3 band-limit IIRs, carrier mix -> analog crt_ntsc.c:254-324
 //   k_mod_nes           PPU pixels -> square-wave IRE sums                 crt_nes.c:21-61, 81-201
-//   k_noise             analog + LCG noise -> inp                          crt_core.c:346-367
-//   k_sync              vsync search, hsync / burst-lock chain, line table crt_core.c:379-479
+//   k_sync              vsync search, hsync / burst-lock chain, line table crt_core.c:379-479;
+//                       LCG noise, analog -> inp                           crt_core.c:346-367
 //   k_lines             Y/I/Q equalisers, resample, YIQ->RGB, blend, store crt_core.c:511-664
 //
 // Everything is int32 fixed point with two's-complement wrap and arithmetic right shift, as the
@@ -196,7 +196,6 @@ __global__ void __launch_bounds__(256) k_mod_skeleton_rgb(const SrcCfg *__restri
                                                           MonState *__restrict__ states,
                                                           signed char *__restrict__ analog_base, int first)
 {
-    grid_dep_launch(); // the picture kernel behind this one may be scheduled as SMs free up (it waits before it writes)
     const SrcCfg s = srcs[blockIdx.x];
     signed char *analog = analog_base + (size_t) (first + blockIdx.x) * kSignalBytes;
     __shared__ int burst[kVper][kCc];
@@ -468,11 +467,8 @@ template <int CR, int CG, int CB, int RP, int GP, int BP> struct YiqDot {
 template <int FMT, bool COLOR>
 __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg *__restrict__ srcs,
                                                                    const MonCfg *__restrict__ cfgs,
-                                                                   signed char *__restrict__ analog_base, int first,
-                                                                   int use_tma)
+                                                                   signed char *__restrict__ analog_base, int first)
 {
-    grid_dep_launch();
-    grid_dep_wait(); // (programmatic launch behind the skeleton kernel: its bytes must be in place first, crt_ntsc.c:205-324)
     phase_mark(2, 0);
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -519,14 +515,12 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
     const int y0 = warp * 32;
     if (y0 >= desth) return;
     const int nlines = min(32, desth - y0);
-    if (use_tma == 1) {
-        if (lane == 0) {
-            mbar_init(&bars[0], 1);
-            mbar_init(&bars[1], 1);
-            mbar_fence_init();
-        }
-        __syncwarp();
+    if (lane == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        mbar_fence_init();
     }
+    __syncwarp();
     const int field = s.field & 1, frame = s.frame & 1;
     const int flip = (field == frame);
     const int ph = kRowCarrier ? 1 : (flip ? -1 : 1); // the template system and the PV-1000 walk colour rows instead (below)
@@ -559,11 +553,6 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
     if (row >= s.h) row = s.h - 1;
     if (s.compact) row = y; // crtx_frames_host staged exactly those rows, in line order (k_rows_gather)
     const unsigned char *rowp = data + (size_t) row * s.w * bpp;
-    // cp.async staging copies the warp's spans four lanes to a row, eight rows at a time: the source rows of lines
-    // 8j + lane / 4, j = 0 .. 3
-    unsigned long long rowoffs[4];
-#pragma unroll
-    for (int j = 0; j < 4; j++) rowoffs[j] = __shfl_sync(0xffffffffu, (unsigned long long) row * s.w * bpp, j * 8 + (lane >> 2));
 
     // chunk c covers samples [32c, 32c + 32); its span of source columns f0..f1 is staged from the 16-byte aligned address
     // at or below pixel f0.  Returns the offset of pixel f0 from that address.
@@ -574,35 +563,13 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
         const int a = (int) (reinterpret_cast<uintptr_t>(p) & 15);
         const unsigned copy = (unsigned) ((a + bytes + 15) & ~15);
         unsigned char *dst = stage + (c & 1) * 32 * kModSRow + lane * kModSRow;
-        if (use_tma == 2) {
-            // 16-byte asynchronous copies, one group per chunk.  Four neighbouring lanes fetch neighbouring 16-byte pieces
-            // of one row, so a copy instruction touches eight rows' spans instead of 32.
+        // rows may sit at different 16-byte phases, so the copies differ in size: sum them up
+        unsigned total = active ? copy : 0;
 #pragma unroll
-            for (int j = 0; j < 4; j++) {
-                const int r = j * 8 + (lane >> 2);
-                const unsigned char *pr = data + rowoffs[j] + (size_t) sp.x * bpp;
-                const int ar = (int) (reinterpret_cast<uintptr_t>(pr) & 15);
-                const unsigned copyr = (unsigned) ((ar + bytes + 15) & ~15);
-                unsigned char *dr = stage + (c & 1) * 32 * kModSRow + r * kModSRow;
-#pragma unroll
-                for (unsigned k = 0; k < (kModSRow / 16 + 3) / 4; k++) {
-                    const unsigned q = k * 4 + (lane & 3);
-                    if (r < nlines && q * 16 < copyr) cp_async_16(dr + q * 16, pr - ar + q * 16);
-                }
-            }
-            cp_async_commit();
-        } else if (use_tma) {
-            // rows may sit at different 16-byte phases, so the copies differ in size: sum them up
-            unsigned total = active ? copy : 0;
-#pragma unroll
-            for (int d = 16; d > 0; d >>= 1) total += __shfl_xor_sync(0xffffffffu, total, d);
-            if (lane == 0) mbar_expect_tx(&bars[c & 1], total);
-            __syncwarp();
-            if (active) tma_load_1d(dst, p - a, copy, &bars[c & 1]);
-        } else if (active) {
-            for (unsigned q = 0; q < copy / 16; q++)
-                reinterpret_cast<uint4 *>(dst)[q] = __ldg(reinterpret_cast<const uint4 *>(p - a) + q);
-        }
+        for (int d = 16; d > 0; d >>= 1) total += __shfl_xor_sync(0xffffffffu, total, d);
+        if (lane == 0) mbar_expect_tx(&bars[c & 1], total);
+        __syncwarp();
+        if (active) tma_load_1d(dst, p - a, copy, &bars[c & 1]);
         return a;
     };
 
@@ -611,7 +578,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
     YiqDot<39059, -18022, -21103, rp, gp, bp> dot_i;
     YiqDot<13894, -34275, 20382, rp, gp, bp> dot_q;
     if (bpp == 4) {
-        const unsigned zero = (unsigned) use_tma >> 8; // (0: the staging mode is 0, 1 or 2)
+        const unsigned zero = (unsigned) first >> 31; // (0: the host keeps first in [0, 2^31))
         dot_y.init(zero);
         if (color) {
             dot_i.init(zero);
@@ -651,12 +618,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
     for (int c = 0; c < nchunks; c++) {
         const int a_nxt = (c + 1 < nchunks) ? issue(c + 1) : 0;
         const int c0 = c * kModSChunk;
-        if (use_tma == 2) { // every lane's copies but those of the chunk just requested have landed (visible to all after the __syncwarp)
-            if (c + 1 < nchunks) cp_async_wait<1>();
-            else cp_async_wait<0>();
-        } else if (use_tma) {
-            mbar_wait(&bars[c & 1], (c >> 1) & 1);
-        }
+        mbar_wait(&bars[c & 1], (c >> 1) & 1);
         __syncwarp();
         const unsigned char *srow = stage + (c & 1) * 32 * kModSRow + lane * kModSRow + a_cur;
         a_cur = a_nxt;
@@ -1048,58 +1010,13 @@ __global__ void __launch_bounds__(256) k_mod_nesrgb(const SrcCfg *__restrict__ s
 #endif // NES-RGB
 
 // =======================================================================================
-// noise pass (crt_core.c:346-367), LCG variant.  16 samples per thread, 128-bit accesses;
+// noise pass (crt_core.c:346-367), LCG variant, run inside k_sync.  16 samples per vector, 128-bit accesses;
 // the generator state of sample i is rn0 advanced i + 1 steps, reached by two table look-ups.
 // =======================================================================================
 constexpr int kNoiseVec = 16;
-constexpr int kNoiseThreads = (kInputSize + kNoiseVec - 1) / kNoiseVec;
-constexpr int kNoiseBlocks = (kNoiseThreads + 255) / 256;
+constexpr int kNoiseThreads = (kInputSize + kNoiseVec - 1) / kNoiseVec; // 16-sample vectors of inp[]
 constexpr int kJumpLo = 128; // lo[k] = jump(16 * k), hi[k] = jump(16 * 128 * k)
 constexpr int kJumpHi = (kNoiseThreads + kJumpLo - 1) / kJumpLo + 1;
-
-__global__ void __launch_bounds__(256) k_noise(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states,
-                                               const signed char *__restrict__ analog_base,
-                                               signed char *__restrict__ inp_base,
-                                               const Affine *__restrict__ jump_lo,
-                                               const Affine *__restrict__ jump_hi, int first)
-{
-    const int m = first + blockIdx.y;
-    const int t = blockIdx.x * 256 + threadIdx.x;
-    const int i0 = t * kNoiseVec;
-    if (i0 >= kInputSize) return;
-    if (cfgs[m].bpp == 0) return; // crt_core.c:312-315: nothing at all happens
-    const int noise = cfgs[m].noise;
-    const signed char *analog = analog_base + (size_t) m * kSignalBytes;
-    signed char *inp = inp_base + (size_t) m * kSignalBytes;
-
-    uint4 in = *reinterpret_cast<const uint4 *>(analog + i0);
-    unsigned w[4] = { in.x, in.y, in.z, in.w };
-    if (noise == 0) {
-#pragma unroll
-        for (int k = 0; k < 4; k++) w[k] = __vmaxs4(w[k], 0x81818181u); // clamp -128 -> -127
-    } else {
-        const Affine lo = jump_lo[t % kJumpLo], hi = jump_hi[t / kJumpLo];
-        unsigned rn = ((unsigned) states[m].rn * hi.mul + hi.add) * lo.mul + lo.add;
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-            unsigned o = 0;
-#pragma unroll
-            for (int b = 0; b < 4; b++) {
-                rn = rn * kLcgMul + kLcgAdd;
-                int a = (int) (signed char) (w[k] >> (8 * b));
-                int s = a + (wmul((int) ((rn >> 16) & 0xff) - 0x7f, noise) >> 8);
-                s = clampi(s, -127, 127);
-                o |= ((unsigned) s & 0xffu) << (8 * b);
-            }
-            w[k] = o;
-        }
-    }
-    if (i0 + kNoiseVec <= kInputSize) {
-        *reinterpret_cast<uint4 *>(inp + i0) = make_uint4(w[0], w[1], w[2], w[3]);
-    } else {
-        for (int b = 0; i0 + b < kInputSize; b++) inp[i0 + b] = (signed char) (w[b >> 2] >> (8 * (b & 3)));
-    }
-}
 
 #if (CRT_SYSTEM == CRT_SYSTEM_NTSCVHS)
 // VHS noise pass with the per-sample noise term drawn elsewhere (crt_core.c:343-366): the drop-in

@@ -141,8 +141,6 @@ constexpr int kMaxOutw = 8192;
 
 struct LinesGeom { // uniform over a launch: host groups monitors by these (crtx.cu)
     int outw, out_format, bpp, blend;
-    int use_tma;
-    int stage2; // k_lines2 only: 0 plain loads, 1 one bulk copy per lane and stage, 2 cp.async (crt_lines2.cuh)
     int pass; // -1: every line; -2: only the last line of each shared-row run; >= 0: lines at this run position
     int rnd; // 32768, passed as an argument so that it lives in a register (see pole())
     int dx;  // ((AV_LEN - 1) << 12) / outw (crt_core.c:527), computed by the host: no division in the kernels
@@ -248,7 +246,6 @@ __global__ void __launch_bounds__(kLinesWarps * 32, (FAST && kCc == 4) ? 2 : 1) 
 k_lines(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, const LineRec *__restrict__ lines_base,
         const signed char *__restrict__ inp_base, int first, const LinesGeom geo)
 {
-    grid_dep_wait(); // (programmatic launch behind k_sync / k_lines2)
     extern __shared__ __align__(128) unsigned char smem_raw[];
     constexpr int kWarpSmem = lines_warp_smem<FAST>();
     constexpr int kEntry = YiqRow<FAST>::kEntryBytes;
@@ -261,14 +258,12 @@ k_lines(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, co
     unsigned *tile = reinterpret_cast<unsigned *>(stage + 2 * kStageBytes);
     unsigned char *yiq = stage + 2 * kStageBytes + kTileBytes + lane * (YiqRow<FAST>::kPitch * kEntry);
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + kLinesWarps * kWarpSmem) + 2 * warp;
-    if (geo.use_tma) {
-        if (lane == 0) {
-            mbar_init(&bars[0], 1);
-            mbar_init(&bars[1], 1);
-            mbar_fence_init();
-        }
-        __syncwarp();
+    if (lane == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        mbar_fence_init();
     }
+    __syncwarp();
 
     const int kline = warp * 32 + lane; // decoded line of this lane
     LineRec rec;
@@ -330,15 +325,9 @@ k_lines(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, co
 
     auto issue = [&](int c) {
         unsigned char *dst = stage + (c & 1) * kStageBytes + lane * kStageRow;
-        if (geo.use_tma) {
-            if (lane == 0) mbar_expect_tx(&bars[c & 1], nactive * kStageRow);
-            __syncwarp();
-            if (active) tma_load_1d(dst, src + c * kStageSamples, kStageRow, &bars[c & 1]);
-        } else if (active) { // plain 16-byte loads, kept for A/B testing of the TMA path
-#pragma unroll
-            for (int q = 0; q < kStageRow / 16; q++)
-                reinterpret_cast<uint4 *>(dst)[q] = __ldg(reinterpret_cast<const uint4 *>(src + c * kStageSamples) + q);
-        }
+        if (lane == 0) mbar_expect_tx(&bars[c & 1], nactive * kStageRow);
+        __syncwarp();
+        if (active) tma_load_1d(dst, src + c * kStageSamples, kStageRow, &bars[c & 1]);
     };
 
     // slot access.  FAST stores {Y, I | Q << 16} with Y NOT yet scaled by 16: there
@@ -391,8 +380,7 @@ k_lines(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, co
 #pragma unroll 1
     for (int c = 0; c < kNumStages; c++) {
         if (c + 1 < kNumStages) issue(c + 1); // the other buffer was drained in iteration c - 1
-        if (geo.use_tma) mbar_wait(&bars[c & 1], (c >> 1) & 1);
-        else __syncwarp();
+        mbar_wait(&bars[c & 1], (c >> 1) & 1);
         const signed char *row = row_base + (c & 1) * kStageBytes;
         const int ns = min(kStageSamples, kSamplesPadded - c * kStageSamples); // a multiple of kSub
 #pragma unroll 1

@@ -20,9 +20,9 @@
 // so "sample s + 1" is always the next slot; a block of 8 pixels is emitted as soon as its last sample is in the
 // ring, which the host guarantees is before its first one is overwritten (7 * dx <= 10 * 4096).
 // Nothing in the loops waits on DRAM with a register: the signal windows arrive by per-lane asynchronous copies (48
-// bytes per lane and stage: cp.async, or one bulk copy per lane -- `use_tma` 2 / 1), the previous image's pixels of the
-// NEXT tile by cp.async into shared memory while the current tile is being computed, and all shared-memory traffic of
-// the hot loops goes through 32-bit shared addresses held in registers.
+// bytes per lane and stage: three 16-byte cp.async), the previous image's pixels of the NEXT tile by cp.async into
+// shared memory while the current tile is being computed, and all shared-memory traffic of the hot loops goes through
+// 32-bit shared addresses held in registers.
 #pragma once
 
 #include "crt_lines.cuh"
@@ -53,7 +53,7 @@ static_assert(kL2RingPitch % 2 == 1, "ring pitch");
 __host__ __device__ constexpr int lines2_desc_count(int outw) { return ((outw + 15) / 16) * 16; }
 __host__ __device__ constexpr int lines2_smem(int outw)
 {
-    return kL2Warps * kL2WarpSmem + kL2Warps * 2 * 8 + lines2_desc_count(outw) * 16;
+    return kL2Warps * kL2WarpSmem + lines2_desc_count(outw) * 16;
 }
 static_assert(lines2_smem(kL2MaxOutw) <= 227 * 1024, "k_lines2 shared memory");
 
@@ -115,9 +115,8 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint4 *desc = reinterpret_cast<uint4 *>(smem_raw + kL2Warps * kL2WarpSmem + kL2Warps * 2 * 8);
+    uint4 *desc = reinterpret_cast<uint4 *>(smem_raw + kL2Warps * kL2WarpSmem);
     const int dx = geo.dx;
-    grid_dep_launch();
     phase_mark(1, 0);
 
     // ---- descriptor table, once per CTA (pixels past outw repeat the last one: they are computed and never stored)
@@ -127,9 +126,6 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
         const unsigned s = npos >> 12, R = npos & 0xfffu;
         desc[k] = make_uint4(4u * R, 4u * (0xfffu - R), (s % (unsigned) kL2Ring) * 8u, s + 1u);
     }
-    // (programmatic launch behind k_sync: everything above depends on the kernel arguments only and runs while k_sync's
-    // last CTAs finish; the line table, the state records and inp[] are read below)
-    grid_dep_wait();
     __syncthreads();
     phase_mark(1, 1);
 
@@ -141,7 +137,6 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
     const int m = first + (present ? mrel : 0);
 
     unsigned char *stage = smem_raw + warp * kL2WarpSmem;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + kL2Warps * kL2WarpSmem) + 2 * warp;
     // 32-bit shared-space addresses of everything the hot loops touch
     const unsigned stage_a = smem_u32(stage);
     const unsigned tile_a = stage_a + 2 * kL2StageBytes;
@@ -150,15 +145,6 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
     const unsigned yiq_a = tile_a + kTileBytes + lane * (kL2RingPitch * 8);
     const unsigned old_a = tile_a + kTileBytes + kL2RingBytes + lane * 16;
     const unsigned desc_a = smem_u32(desc);
-    const int staging = geo.stage2; // 0: plain loads, 1: one bulk copy (TMA) per lane and stage, 2: cp.async per lane
-    if (staging == 1) {
-        if (lane == 0) {
-            mbar_init(&bars[0], 1);
-            mbar_init(&bars[1], 1);
-            mbar_fence_init();
-        }
-        __syncwarp();
-    }
 
     LineRec rec;
     rec.pos = 0; rec.wave0 = rec.wave1 = 0; rec.beg = -1; rec.end = -1; rec.hsync = 0; rec.pad0 = rec.pad1 = 0;
@@ -166,7 +152,6 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
     const bool active = present && states[m].generic == 0 && rec.beg >= 0 && kline >= geo.line_lo && kline < geo.line_hi;
     const unsigned active_mask = __ballot_sync(0xffffffffu, active);
     if (active_mask == 0) return;
-    const unsigned nactive = __popc(active_mask);
 
     const MonCfg *cfg = &cfgs[m];
     const int contrast = cfg->contrast;
@@ -211,21 +196,11 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
     auto issue = [&](int c) { // request stage c: samples [c * kL2Stage, + kL2Stage) of every active lane's window
         unsigned char *dst = stage + (c & 1) * kL2StageBytes + lane * kL2StageRow;
         const signed char *src = inp + ((rec.pos + c * kL2Stage) & ~15);
-        if (staging == 1) {
-            if (lane == 0) mbar_expect_tx(&bars[c & 1], nactive * kL2StageRow);
-            __syncwarp();
-            if (active) tma_load_1d(dst, src, kL2StageRow, &bars[c & 1]);
-        } else if (staging == 2) {
-            if (active) {
+        if (active) {
 #pragma unroll
-                for (int q = 0; q < kL2StageRow / 16; q++) cp_async_16(dst + 16 * q, src + 16 * q);
-            }
-            cp_async_commit();
-        } else if (active) { // plain 16-byte loads, kept for A/B testing
-#pragma unroll
-            for (int q = 0; q < kL2StageRow / 16; q++)
-                reinterpret_cast<uint4 *>(dst)[q] = __ldg(reinterpret_cast<const uint4 *>(src) + q);
+            for (int q = 0; q < kL2StageRow / 16; q++) cp_async_16(dst + 16 * q, src + 16 * q);
         }
+        cp_async_commit();
     };
 
     Eq ey, ei, eq;
@@ -250,8 +225,7 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
 #pragma unroll 1
     for (int c = 0; c < kL2Stages; c++) {
         // stage c has had a whole stage of work to arrive
-        if (staging == 1) mbar_wait(&bars[c & 1], (c >> 1) & 1);
-        else if (staging == 2) cp_async_wait<0>();
+        cp_async_wait<0>();
         __syncwarp(); // ... and every lane is done with the other buffer, which is refilled now
         if (c + 1 < kL2Stages) issue(c + 1);
         const signed char *row = row_base + (c & 1) * kL2StageBytes + ((rec.pos + c * kL2Stage) & 15);
@@ -318,7 +292,7 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
         const int k0 = (blk - 1) * kL2Block;
         flush_tile<MODE == 1>(tile_q_a, old_a, tr, pitch, geo.outw - k0, 0, lane, blend_mask);
     }
-    if (staging == 2 || MODE == 1) cp_async_wait<0>();
+    cp_async_wait<0>();
     phase_mark(1, 14);
     phase_mark(1, 12, 7 * 32);
 }

@@ -105,7 +105,6 @@ __global__ void __launch_bounds__(kFirWarps * 32, FAST ? 2 : 1)
 k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, const LineRec *__restrict__ lines_base,
             const signed char *__restrict__ inp_base, int first, const LinesGeom geo)
 {
-    grid_dep_wait(); // (programmatic launch behind k_sync)
     extern __shared__ __align__(128) unsigned char smem_raw[];
     using Elem = typename FirRow<FAST>::Elem;
     constexpr int kComp = FirRow<FAST>::kCompBytes / (int) sizeof(Elem); // elements between the Y, I and Q rows
@@ -164,7 +163,7 @@ k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states
     const int pitch = geo.outw * bpp;
     // rows go through shared memory and bulk copies when they are 16-byte granular; otherwise (3-byte
     // pixels, odd widths, unaligned images) every lane reads and writes its own pixels
-    const bool bulk = (MODE != 2) && geo.use_tma && ((geo.outw & 3) == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
+    const bool bulk = (MODE != 2) && ((geo.outw & 3) == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
     const bool prefetch_old = bulk && (MODE == 1);
     const signed char *inp = inp_base + (size_t) m * kSignalBytes;
     const unsigned dx = (unsigned) (((kAvLen - 1) << 12) / geo.outw); // crt_core.c:527
@@ -205,7 +204,7 @@ k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states
         tab_k0 = 0;
     }
 
-    if (geo.use_tma && lane == 0 && is_active(cur)) {
+    if (lane == 0 && is_active(cur)) {
         request_signal(cur, 0);
         if (prefetch_old) request_old(cur, 0, 0, seg0);
     }
@@ -215,7 +214,7 @@ k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states
         const int buf = it & 1;
         // line n + 1's signal window and line n + 2's record
         const bool nxt_active = is_active(nxt); // (fetched a whole line ago)
-        if (geo.use_tma && lane == 0 && nxt_active) request_signal(nxt, buf ^ 1);
+        if (lane == 0 && nxt_active) request_signal(nxt, buf ^ 1);
         const FirLine nn = fetch(kline + 2 * stride);
 
         if (is_active(cur)) {
@@ -223,15 +222,8 @@ k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states
             const int a = cur.pos & 15;
             const int nrows = max(1, cur.end - scanlines - cur.beg); // crt_core.c:662-664
             unsigned char *row0 = out + (size_t) cur.beg * pitch;
-            if (geo.use_tma) {
-                mbar_wait(&bars[buf], (ph_sig >> buf) & 1);
-                ph_sig ^= 1u << buf;
-            } else {
-                const signed char *src = inp + (cur.pos & ~15);
-                for (int q = lane; q < kFirStage / 16; q += 32)
-                    reinterpret_cast<uint4 *>(sigbuf)[q] = __ldg(reinterpret_cast<const uint4 *>(src) + q);
-                __syncwarp();
-            }
+            mbar_wait(&bars[buf], (ph_sig >> buf) & 1);
+            ph_sig ^= 1u << buf;
             const int nw0 = wsub(0, cur.wave0), nw1 = wsub(0, cur.wave1);
             // wave[(i + 0) & 3] feeds I, wave[(i + 3) & 3] feeds Q (crt_core.c:538-543)
             const int wi[4] = { cur.wave0, cur.wave1, nw0, nw1 };

@@ -6,7 +6,6 @@
 
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <string.h>
 
 namespace crt {
 
@@ -61,11 +60,6 @@ __device__ __forceinline__ void tma_load_1d(void *dst, const void *src, unsigned
 __device__ __forceinline__ void cp_async_16(void *dst, const void *src)
 {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
-}
-// 4-byte flavour (.ca: the only cache operator the small sizes have)
-__device__ __forceinline__ void cp_async_4(void *dst, const void *src)
-{
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int PENDING> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(PENDING) : "memory"); }
@@ -123,14 +117,6 @@ __device__ __forceinline__ void cp_async_16a(unsigned dst_addr, const void *src)
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst_addr), "l"(src) : "memory");
 }
 
-// Programmatic dependent launch (sm_90+): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may be
-// scheduled while its predecessor in the stream is still running -- its CTAs take SMs as the predecessor's CTAs leave them and
-// run whatever depends on kernel arguments only -- and `grid_dep_wait` holds it until the predecessor grid has completed and
-// its memory is visible.  `grid_dep_launch` is the predecessor's side: "my dependents may be scheduled now".  Both are
-// no-ops in a kernel that was launched the ordinary way.
-__device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
 // Two-way dot product of 16-bit by 8-bit values with 32-bit accumulate (IDP.2A): a holds two 16-bit values (signed when
 // SIGNED_A, else unsigned), b four unsigned bytes of which the low (HI = false: bytes 0, 1) or the high pair (bytes 2, 3)
 // takes part:  c + a.h0 * b.byte[0 | 2] + a.h1 * b.byte[1 | 3]  (mod 2^32).
@@ -178,30 +164,6 @@ template <typename Elem, int OFF> __device__ __forceinline__ int lds_elem(unsign
     if (sizeof(Elem) == 2) asm volatile("ld.shared.s16 %0, [%1+%2];" : "=r"(v) : "r"(addr), "n"(OFF));
     else asm volatile("ld.shared.s32 %0, [%1+%2];" : "=r"(v) : "r"(addr), "n"(OFF));
     return v;
-}
-
-// ---------------------------------------------------------------------------------------
-// host side of the same feature
-// ---------------------------------------------------------------------------------------
-// Launch `kernel`; with `pdl` as a programmatic dependent of the kernel launched just before it on `stream`: it may be
-// scheduled while that one is still running and waits for it inside (grid_dep_wait, crt_ptx.cuh).  Only kernels that call
-// grid_dep_wait before their first read of global memory are launched this way.
-template <typename... KA, typename... A>
-inline cudaError_t launch_kernel(bool pdl, void (*kernel)(KA...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, A &&...args)
-{
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    memset(attr, 0, sizeof(attr));
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl ? 1u : 0u;
-    return cudaLaunchKernelEx(&cfg, kernel, static_cast<KA>(args)...);
 }
 
 } // namespace crt

@@ -63,7 +63,7 @@ struct SyncShared {
     int rowcount[kVper > 3 ? kVper : 3];
     int vs_found[2 * kVsyncWindow]; // per vsync candidate: crossing index or -1
     int generic;
-    int noise_next; // next chunk of the noise pass to hand out (FUSED)
+    int noise_next; // next chunk of the noise pass to hand out (kFusedNoise)
     int need_max;   // some line of this pass needed its signal lines' largest sample
     int linemax[kVres + 2]; // largest |sample| of each signal line of inp[], measured by the noise pass when MonState::track_max says so
 };
@@ -178,11 +178,12 @@ __device__ __forceinline__ unsigned clamp127_4(unsigned x)
     return x | ((x & ~nz & 0x80808080u) >> 7);
 }
 
-// FUSED (LCG systems): the kernel reads analog[], applies the noise itself to what it stages, and writes the whole
-// inp[] -- the separate noise pass disappears.  That copy is pure memory traffic and the burst-lock chain pure latency on one
+// The LCG systems' noise pass is fused into this kernel (kFusedNoise): it reads analog[], applies the noise itself to what it
+// stages, and writes the whole inp[].  That copy is pure memory traffic and the burst-lock chain pure latency on one
 // warp, so they overlap: while the last warp runs the chain the other seven copy, 4 KB chunks handed out by a counter in shared
 // memory (the chain warp joins when it is through).
-// !FUSED (VHS, whose noise comes from rand()): inp[] was written by k_noise_vhs.
+// VHS, whose noise comes from rand(): inp[] was written by k_noise_vhs, and this kernel reads it.
+constexpr bool kFusedNoise = !kIsVhs;
 constexpr int kNoiseNB = 8;                                   // 16-byte loads in flight per thread
 constexpr int kNoiseChunkVecs = 32 * kNoiseNB;                // vectors per chunk (one warp, kNoiseNB rounds)
 constexpr int kNoiseChunks = (kNoiseThreads + kNoiseChunkVecs - 1) / kNoiseChunkVecs;
@@ -196,7 +197,6 @@ constexpr int kCandVecs = (12 + 4 * kCandWords + 15) / 16;
 constexpr int kStageVecs = kHeadLines * kHeadVecs + 2 * kVsyncWindow * kCandVecs;
 constexpr int kStageBatch = (kStageVecs + kSyncThreads - 1) / kSyncThreads; // vector loads per thread, all in flight at once
 
-template <bool FUSED>
 __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restrict__ cfgs, MonState *__restrict__ states,
                                                           LineRec *__restrict__ lines_base,
                                                           const signed char *__restrict__ analog_base,
@@ -205,8 +205,6 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
                                                           const Affine *__restrict__ jump_hi, int first,
                                                           int force_generic)
 {
-    grid_dep_launch();
-    grid_dep_wait(); // (programmatic launch behind the encoder: analog[] must be complete)
     phase_mark(0, 0);
     extern __shared__ __align__(16) unsigned heads[]; // [kHeadLines][kHeadWords]
     __shared__ SyncShared sh;
@@ -216,20 +214,20 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
     MonState *st = &states[m];
     const signed char *analog = analog_base + (size_t) m * kSignalBytes;
     signed char *inp_w = inp_base + (size_t) m * kSignalBytes;
-    const signed char *inp = inp_w; // !FUSED reads; fall-back loads when sync is lost (see below)
+    const signed char *inp = inp_w; // VHS reads; fall-back loads when sync is lost (see below)
     LineRec *lines = lines_base + (size_t) m * kLines;
     const unsigned rn0 = (unsigned) st->rn;
     const int noise = cfg.noise;
     auto fetch = [&](int p) { // one staged word
         if (p < 0) return 0u;
-        if (FUSED) return noisy_word(analog, p, noise, rn0, jump_lo, jump_hi);
+        if (kFusedNoise) return noisy_word(analog, p, noise, rn0, jump_lo, jump_hi);
         return __ldg(reinterpret_cast<const unsigned *>(inp + p));
     };
     auto fetch_byte = [&](int p) { // a single sample outside the staged regions (sync lost)
         const unsigned w = fetch(p & ~3);
         return (int) (signed char) (w >> (8 * (p & 3)));
     };
-    const int track = FUSED ? st->track_max : 0; // measure every signal line's largest sample during the copy (see step 4)
+    const int track = kFusedNoise ? st->track_max : 0; // measure every signal line's largest sample during the copy (see step 4)
     if (tid == 0) {
         sh.noise_next = 0;
         sh.need_max = 0;
@@ -247,7 +245,7 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
     const int cand0 = posmod(vs_in - kVsyncWindow, kVres);
     auto cand_line = [&](int c) { return (cand0 + c >= kVres) ? cand0 + c - kVres : cand0 + c; };
     {
-        const signed char *from = FUSED ? analog : inp;
+        const signed char *from = kFusedNoise ? analog : inp;
         // where staged vector idx comes from and which row words it feeds (computed twice -- for the load and again for the
         // stores -- rather than kept: with every load of the phase in flight at once the registers belong to the data)
         auto place = [&](int idx, int &pos, int &w0, int &nw) -> unsigned * {
@@ -284,7 +282,7 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
             unsigned *row = place(b * kSyncThreads + tid, pos, w0, nw);
             if (nw == 0) continue;
             unsigned w[4] = { v[b].x, v[b].y, v[b].z, v[b].w };
-            if (FUSED && pos >= 0) {
+            if (kFusedNoise && pos >= 0) {
                 if (noise == 0 && pos + 16 <= kInputSize) {
 #pragma unroll
                     for (int e = 0; e < 4; e++) w[e] = clamp127_4(w[e]);
@@ -516,7 +514,7 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
     }
     // ---- 3c. the noise pass proper (crt_core.c:346-367): analog -> inp, 16 samples per thread per round, 128-bit accesses,
     // by the seven warps that would otherwise wait for the chain (which joins them when it is through)
-    if (FUSED) {
+    if (kFusedNoise) {
         for (;;) {
             int c = 0;
             if (lane == 0) c = atomicAdd(&sh.noise_next, 1);
@@ -653,7 +651,7 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
             // burst-lock chain; the first pass of such a monitor scans the two lines here instead, one thread per line, slowly.
             const int stail = (rec.pos + kAvLen > kInputSize) ? 128 : 0;
             int smax = max(127, stail);
-            if (FUSED && ((smax * wmax) >> 9) + 1 > 16383) {
+            if (kFusedNoise && ((smax * wmax) >> 9) + 1 > 16383) {
                 sh.need_max = 1; // (the next pass of this monitor measures while it copies)
                 if (track) {
                     smax = max(sh.linemax[g.ypos], sh.linemax[g.ypos + 1]);
@@ -672,7 +670,7 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
     __syncthreads();
     if (tid == 0) {
         st->generic = sh.generic;
-        if (FUSED) st->track_max = sh.need_max;
+        if (kFusedNoise) st->track_max = sh.need_max;
     }
     phase_mark(0, 14);
 }

@@ -81,13 +81,11 @@ static void launch_lines_one(crtx_ctx *ctx, int count, int lo, const LinesGeom &
         int gx = FAST ? (4 * ctx->sm_count + count - 1) / count : 1;
         gx = gx < 1 ? 1 : (gx > kFirGroups ? kFirGroups : gx);
         const dim3 grid(gx, count);
-        (void) launch_kernel(ctx->opt_pdl != 0, k_lines_fir<FAST, MODE, FMT>, grid, dim3(kFirWarps * 32), (size_t) fir_smem<FAST>(), stream,
-                             (const MonCfg *) ctx->d_cfg, (const MonState *) ctx->d_state, (const LineRec *) ctx->d_lines,
-                             (const signed char *) ctx->d_inp, lo, geo);
+        k_lines_fir<FAST, MODE, FMT><<<grid, kFirWarps * 32, fir_smem<FAST>(), stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines,
+                                                                                      ctx->d_inp, lo, geo);
     } else { // (only the kernel a build uses is instantiated)
-        (void) launch_kernel(ctx->opt_pdl != 0, k_lines<FAST, MODE, FMT>, dim3(count), dim3(kLinesWarps * 32), (size_t) lines_smem<FAST>(), stream,
-                             (const MonCfg *) ctx->d_cfg, (const MonState *) ctx->d_state, (const LineRec *) ctx->d_lines,
-                             (const signed char *) ctx->d_inp, lo, geo);
+        k_lines<FAST, MODE, FMT><<<count, kLinesWarps * 32, lines_smem<FAST>(), stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines,
+                                                                                       ctx->d_inp, lo, geo);
     }
 }
 
@@ -121,9 +119,8 @@ static bool lines2_eligible(const crtx_ctx *ctx, int count, int lo, const LinesG
 template <int MODE, int FMT>
 static void launch_lines2_one(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo, cudaStream_t stream)
 {
-    (void) launch_kernel(ctx->opt_pdl != 0, k_lines2<MODE, FMT>, dim3((count + 1) / 2), dim3(kL2Threads), (size_t) lines2_smem(geo.outw), stream,
-                         (const MonCfg *) ctx->d_cfg, (const MonState *) ctx->d_state, (const LineRec *) ctx->d_lines,
-                         (const signed char *) ctx->d_inp, lo, count, geo);
+    k_lines2<MODE, FMT><<<(count + 1) / 2, kL2Threads, lines2_smem(geo.outw), stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines,
+                                                                                          ctx->d_inp, lo, count, geo);
 }
 
 static void launch_lines2(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo, cudaStream_t stream)
@@ -201,10 +198,7 @@ static cudaError_t lines_attr_all()
 template <int FMT, bool COLOR>
 static void launch_mod_staged_one(crtx_ctx *ctx, int count, int first, cudaStream_t stream)
 {
-    // staging: 1 = per-lane bulk copies (default), 2 = per-lane cp.async copies ("mod_bulk" 0), 0 = plain loads
-    const int staging = ctx->opt_tma ? (ctx->opt_mod_bulk ? 1 : 2) : 0;
-    (void) launch_kernel(ctx->opt_pdl != 0, k_mod_picture_rgb_staged<FMT, COLOR>, dim3(count), dim3(256), (size_t) kModSSmem, stream,
-                         (const SrcCfg *) (ctx->d_src + first), (const MonCfg *) ctx->d_cfg, ctx->d_analog, first, staging);
+    k_mod_picture_rgb_staged<FMT, COLOR><<<count, 256, kModSSmem, stream>>>(ctx->d_src + first, ctx->d_cfg, ctx->d_analog, first);
 }
 
 // function attributes are per device: set by crtx_create for the context's device
@@ -431,37 +425,16 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
         k_vhs_commit<<<(count * 32 + 255) / 256, 256, 0, stream>>>(static_cast<VhsRand *>(ctx->d_vhs_rand),
                                                                    static_cast<const VhsRand *>(ctx->d_vhs_rand_next), first, count);
     }
-    {
-        LaunchTimer lt(ctx, stream, 3);
-        k_sync<false><<<count, kSyncThreads, kSyncSmem, stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines, ctx->d_analog,
-                                                                  ctx->d_inp, ctx->d_jump_lo, ctx->d_jump_hi, first,
-                                                                  ctx->opt_generic);
-    }
     int pre = 2;
 #else
     (void) d_noise_terms;
-    int pre = 1;
-    if (ctx->opt_fused_noise) { // the noise pass runs inside k_sync (crt_sync.cuh)
-        LaunchTimer lt(ctx, stream, 3);
-        // (a programmatic dependent of the encoder only when the encoder's last kernel is right in front of it on this stream:
-        // the batch path's crtx_modulate -> crtx_demodulate; any other predecessor is waited for in full, as always)
-        (void) launch_kernel(ctx->opt_pdl != 0, k_sync<true>, dim3(count), dim3(kSyncThreads), (size_t) kSyncSmem, stream,
-                             (const MonCfg *) ctx->d_cfg, ctx->d_state, ctx->d_lines, (const signed char *) ctx->d_analog,
-                             ctx->d_inp, (const Affine *) ctx->d_jump_lo, (const Affine *) ctx->d_jump_hi, first, ctx->opt_generic);
-    } else {
-        dim3 ngrid(kNoiseBlocks, count);
-        {
-            LaunchTimer lt(ctx, stream, 2);
-            k_noise<<<ngrid, 256, 0, stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_analog, ctx->d_inp, ctx->d_jump_lo,
-                                               ctx->d_jump_hi, first);
-        }
-        LaunchTimer lt(ctx, stream, 3);
-        k_sync<false><<<count, kSyncThreads, kSyncSmem, stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines, ctx->d_analog,
-                                                                  ctx->d_inp, ctx->d_jump_lo, ctx->d_jump_hi, first,
-                                                                  ctx->opt_generic);
-        pre = 2;
-    }
+    int pre = 1; // the noise pass runs inside k_sync (crt_sync.cuh)
 #endif
+    {
+        LaunchTimer lt(ctx, stream, 3);
+        k_sync<<<count, kSyncThreads, kSyncSmem, stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines, ctx->d_analog, ctx->d_inp,
+                                                           ctx->d_jump_lo, ctx->d_jump_hi, first, ctx->opt_generic);
+    }
     if (kBloom) { // line sums and the beam-energy chain: every line's resampling step and first sample
         LaunchTimer lt(ctx, stream, 3);
         k_bloom<<<count, 256, 0, stream>>>(ctx->d_cfg, ctx->d_lines, ctx->d_inp, static_cast<BloomLine *>(ctx->d_bloom), first);
@@ -485,8 +458,6 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
         geo.out_format = c0.out_format;
         geo.bpp = c0.bpp;
         geo.blend = c0.blend ? 1 : 0;
-        geo.use_tma = ctx->opt_tma;
-        geo.stage2 = ctx->opt_tma ? ctx->opt_lines2_stage : 0;
         geo.rnd = 32768;
         geo.dx = c0.outw > 0 ? ((kAvLen - 1) << 12) / c0.outw : 0;
         geo.line_lo = ctx->opt_line_lo;
@@ -775,10 +746,7 @@ int crtx_create(crtx_ctx **out, int n)
     ctx->cfg_dirty_hi = n;
     ctx->tail_dirty_lo = 0;
     ctx->tail_dirty_hi = n;
-    ctx->opt_tma = 1;
     ctx->opt_generic = 0;
-    const char *e = getenv("CRT_B200_NO_TMA");
-    if (e && *e == '1') ctx->opt_tma = 0;
 
 #define CTX_TRY(expr)                                                                            \
     do {                                                                                         \
@@ -840,8 +808,7 @@ int crtx_create(crtx_ctx **out, int n)
 #endif
     CTX_TRY(lines_attr_all());
     CTX_TRY(lines2_attr_all());
-    CTX_TRY(cudaFuncSetAttribute(k_sync<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSyncSmem));
-    CTX_TRY(cudaFuncSetAttribute(k_sync<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSyncSmem));
+    CTX_TRY(cudaFuncSetAttribute(k_sync, cudaFuncAttributeMaxDynamicSharedMemorySize, kSyncSmem));
 #if CRT_B200_BANDLIMITED
     CTX_TRY(cudaFuncSetAttribute(k_mod_picture_rgb, cudaFuncAttributeMaxDynamicSharedMemorySize, kModSmem));
     CTX_TRY(mod_staged_attr_all());
@@ -1310,17 +1277,12 @@ int crtx_sync(void *stream)
 int crtx_set_option(crtx_ctx *ctx, const char *name, int value)
 {
     if (!ctx || !name) return fail("crtx_set_option: bad arguments");
-    if (!strcmp(name, "tma")) ctx->opt_tma = value;
-    else if (!strcmp(name, "generic_eq")) ctx->opt_generic = value;
+    if (!strcmp(name, "generic_eq")) ctx->opt_generic = value;
     else if (!strcmp(name, "timing")) ctx->opt_timing = value;
     else if (!strcmp(name, "mod_staged")) ctx->opt_mod_staged = value;
-    else if (!strcmp(name, "fused_noise")) ctx->opt_fused_noise = value;
     else if (!strcmp(name, "host_src")) ctx->opt_host_src = value;
     else if (!strcmp(name, "host_rows")) ctx->opt_host_rows = value;
-    else if (!strcmp(name, "mod_bulk")) ctx->opt_mod_bulk = value;
-    else if (!strcmp(name, "pdl")) ctx->opt_pdl = value;
     else if (!strcmp(name, "lines2")) ctx->opt_lines2 = value;
-    else if (!strcmp(name, "lines2_stage")) ctx->opt_lines2_stage = value;
     else if (!strcmp(name, "line_lo")) ctx->opt_line_lo = value;
     else if (!strcmp(name, "line_hi")) ctx->opt_line_hi = value;
     else return fail("crtx_set_option: unknown option '%s'", name);

@@ -14,15 +14,15 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "ntsc-crt_b200", "lib")
 
 HOT = {  # variant -> substrings of the kernels worth listing
-    "ntsc": ["k_mod_skeleton_rgb", "k_mod_picture_rgb_stagedILi5ELb1", "k_syncILb1", "k_linesILb1ELi1ELi5", "k_linesILb0ELi1ELi5"],
+    "ntsc": ["k_mod_skeleton_rgb", "k_mod_picture_rgb_stagedILi5ELb1", "6k_syncE", "k_linesILb1ELi1ELi5", "k_linesILb0ELi1ELi5"],
     "ntsc_conv": ["k_lines_firILb1ELi1ELi5", "k_lines_firILb0ELi1ELi5"],
     "ntsc_conv4": ["k_lines_firILb1ELi1ELi5"],
-    "vhs": ["k_noise_vhs", "k_syncILb0"],
+    "vhs": ["k_noise_vhs", "6k_syncE"],
     "nes_p0": ["k_nes_table", "k_mod_nes"],
     "snes": ["k_mod_snes"],
     "nesrgb": ["k_mod_nesrgb"],
-    "template": ["k_mod_skeleton_rgb", "k_mod_picture_rgb_stagedILi5ELb1", "k_syncILb1"],
-    "pv1k": ["k_mod_skeleton_rgb", "k_mod_picture_rgbEPK", "k_syncILb1", "k_linesILb1ELi1ELi5", "k_linesILb0ELi1ELi5"],
+    "template": ["k_mod_skeleton_rgb", "k_mod_picture_rgb_stagedILi5ELb1", "6k_syncE"],
+    "pv1k": ["k_mod_skeleton_rgb", "k_mod_picture_rgbEPK", "6k_syncE", "k_linesILb1ELi1ELi5", "k_linesILb0ELi1ELi5"],
     "ntsc_bloom": ["k_bloom", "k_lines_bloom"],
 }
 

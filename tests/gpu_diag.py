@@ -12,16 +12,15 @@ import support as S
 from ntsc_crt_b200 import capi, layout
 
 
-def stage_check(variant, outw, outh, noise, tma, generic, blend=1, scanlines=1, fields=2):
+def stage_check(variant, outw, outh, noise, generic, blend=1, scanlines=1, fields=2):
     import torch
     spec = layout.system_spec(variant)
-    tag = "%s %dx%d noise=%d tma=%d generic=%d" % (variant, outw, outh, noise, tma, generic)
+    tag = "%s %dx%d noise=%d generic=%d" % (variant, outw, outh, noise, generic)
     print("=== " + tag)
     nes = spec.system == layout.SYS_NES
     img = S.nes_image(seed=5) if nes else S.rand_image(832, 624, seed=3)
     dimg = torch.from_numpy(img.view(np.int16) if nes else img).cuda()
     b = capi.Batch(variant, 1)
-    b.set_option("tma", tma)
     b.set_option("generic_eq", generic)
     out = torch.zeros(outh, outw, 4, dtype=torch.uint8, device="cuda")
     b.set_monitor(0, out, noise=noise, blend=blend, scanlines=scanlines)
@@ -103,16 +102,15 @@ def main():
     variants = sys.argv[1:] or ["ntsc"]
     results = []
     for v in variants:
-        for cfg in [dict(noise=0, tma=0, generic=1), dict(noise=0, tma=0, generic=0),
-                    dict(noise=0, tma=1, generic=0), dict(noise=24, tma=1, generic=0)]:
+        for cfg in [dict(noise=0, generic=1), dict(noise=0, generic=0), dict(noise=24, generic=0)]:
             try:
                 results.append(stage_check(v, 832, 624, **cfg))
             except Exception:
                 traceback.print_exc()
                 results.append(False)
         try:
-            results.append(stage_check(v, 640, 480, 12, 1, 0, blend=0, scanlines=1, fields=3))
-            results.append(stage_check(v, 256, 240, 0, 1, 0, blend=0, scanlines=0, fields=2))
+            results.append(stage_check(v, 640, 480, 12, 0, blend=0, scanlines=1, fields=3))
+            results.append(stage_check(v, 256, 240, 0, 0, blend=0, scanlines=0, fields=2))
         except Exception:
             traceback.print_exc()
             results.append(False)

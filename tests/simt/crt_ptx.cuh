@@ -19,7 +19,6 @@ void mbar_expect_tx(uint64_t *bar, unsigned bytes);
 void mbar_wait(uint64_t *bar, unsigned parity);
 void bulk_load(void *dst, const void *src, unsigned bytes, uint64_t *bar);
 void lane_copy16(void *dst, const void *src);
-void lane_copy4(void *dst, const void *src);
 void lane_commit();
 void lane_wait(int pending);
 void bulk_store(void *dst, const void *src, unsigned bytes);
@@ -39,7 +38,6 @@ __device__ __forceinline__ void tma_load_1d(void *dst, const void *src, unsigned
     ::simt::bulk_load(dst, src, bytes, bar);
 }
 __device__ __forceinline__ void cp_async_16(void *dst, const void *src) { ::simt::lane_copy16(dst, src); }
-__device__ __forceinline__ void cp_async_4(void *dst, const void *src) { ::simt::lane_copy4(dst, src); }
 __device__ __forceinline__ void cp_async_commit() { ::simt::lane_commit(); }
 template <int PENDING> __device__ __forceinline__ void cp_async_wait() { ::simt::lane_wait(PENDING); }
 
@@ -78,9 +76,6 @@ template <bool HI, bool SIGNED_A> __device__ __forceinline__ int dp2a_u8(unsigne
     return (int) ((unsigned) c + h0 * b0 + h1 * b1);
 }
 
-// (kernels run one after the other here: nothing to wait for)
-__device__ __forceinline__ void grid_dep_wait() {}
-__device__ __forceinline__ void grid_dep_launch() {}
 __device__ __forceinline__ void phase_mark(int, int, int = 0) {}
 
 template <typename Elem, int OFF> __device__ __forceinline__ int lds_elem(unsigned addr)
@@ -88,15 +83,6 @@ template <typename Elem, int OFF> __device__ __forceinline__ int lds_elem(unsign
     const unsigned char *p = ::simt::g_smem_anchor + (int) (addr + (unsigned) OFF); // offsets may be "negative"
     if ((uintptr_t) p % sizeof(Elem)) ::simt::ptx_fail("ld.shared: misaligned address");
     return (int) *reinterpret_cast<const Elem *>(p);
-}
-
-// host side: here a kernel always starts after its predecessor has finished, so "programmatic dependent" launches are
-// ordinary ones
-template <typename... KA, typename... A>
-inline cudaError_t launch_kernel(bool, void (*kernel)(KA...), dim3 grid, dim3 block, size_t smem, cudaStream_t, A &&...args)
-{
-    ::simt::launch(grid, block, smem, [&]() { kernel(static_cast<KA>(args)...); });
-    return cudaSuccess;
 }
 
 } // namespace crt

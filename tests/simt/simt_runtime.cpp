@@ -232,11 +232,6 @@ void lane_copy16(void *dst, const void *src)
     if (((uintptr_t) dst & 15) || ((uintptr_t) src & 15)) fatal("cp.async 16: misaligned address");
     g_fiber->lane_open.push_back(Copy{ dst, src, 16u });
 }
-void lane_copy4(void *dst, const void *src)
-{
-    if (((uintptr_t) dst & 3) || ((uintptr_t) src & 3)) fatal("cp.async 4: misaligned address");
-    g_fiber->lane_open.push_back(Copy{ dst, src, 4u });
-}
 void lane_commit()
 {
     g_fiber->lane_groups.push_back(g_fiber->lane_open);

@@ -20,8 +20,9 @@ def test_argument_errors_are_reported_not_ignored():
     assert lib.crtx_create(C.byref(ctx), 0) != 0 and b"crtx_create" in lib.crtx_last_error()
     b = capi.Batch("ntsc", 2)
     out = torch.zeros(48, 64, 4, dtype=torch.uint8, device="cuda")
-    with pytest.raises(capi.CrtxError, match="unknown option"):
-        b.set_option("no_such_option", 1)
+    for name in ("no_such_option", "tma", "fused_noise", "mod_bulk", "lines2_stage", "pdl"):
+        with pytest.raises(capi.CrtxError, match="unknown option"):
+            b.set_option(name, 1)
     with pytest.raises(capi.CrtxError, match="range"):
         b.modulate(first=1, count=2)
     with pytest.raises(capi.CrtxError, match="range"):
@@ -200,12 +201,10 @@ def test_frames_host_moves_only_the_rows_a_field_touches(variant, raw, monkeypat
 
 
 @pytest.mark.parametrize("variant", ["ntsc", "ntsc_conv", "template", "pv1k"])
-@pytest.mark.parametrize("option,value", [("generic_eq", 1), ("mod_staged", 0), ("fused_noise", 0), ("mod_bulk", 0), ("tma", 0),
-                                          ("lines2", 0), ("lines2_stage", 1)])
+@pytest.mark.parametrize("option,value", [("generic_eq", 1), ("mod_staged", 0), ("lines2", 0)])
 def test_every_switch_of_the_library_gives_the_same_bits(variant, option, value):
-    """the A/B switches of crtx_set_option select other code paths (the wrap-exact equaliser on every monitor, the
-    gather encoder, the separate noise kernel, per-lane cp.async staging, plain loads instead of bulk copies): all of
-    them must decode to the oracle's image"""
+    """the switches of crtx_set_option that force a path real inputs also take (the wrap-exact equaliser on every
+    monitor, the gather encoder, k_lines in place of k_lines2): all of them must decode to the oracle's image"""
     import torch
     from ntsc_crt_b200 import capi
     b = capi.Batch(variant, 2)

@@ -121,14 +121,12 @@ def test_conv_other_kernels(variant):
         check(gpu, ora, ref, "%s %dx%d extreme" % (variant, outw, outh))
 
 
-@pytest.mark.parametrize("tma", [1, 0])
-def test_conv_batch_matches_oracle(tma):
+def test_conv_batch_matches_oracle():
     """crtx_* batch interface: independent monitors with different knobs and sources, several fields."""
     import torch
     from ntsc_crt_b200 import capi
     n = 5
     b = capi.Batch(V, n)
-    b.set_option("tma", tma)
     outs, oras, imgs = [], [], []
     for i in range(n):
         t = torch.zeros(480, 640, 4, dtype=torch.uint8, device="cuda")

@@ -362,8 +362,7 @@ def copy_sizes(addr, w, destw, bpp, rows):
 
 
 @pytest.mark.parametrize("variant,destw", [("ntsc", 753), ("ntsc_bloom", 637), ("pv1k", 1487)])
-@pytest.mark.parametrize("staging", ["default", "mod_bulk0", "tma0"])
-def test_staged_encoder_span_edge(variant, destw, staging):
+def test_staged_encoder_span_edge(variant, destw):
     """The widest source the staged encoder accepts and one pixel wider (which the gather encoder takes), 4- and 3-byte
     pixels, scaled and raw, at source addresses that make some chunk copy the whole 176-byte stage row: analog[] equal to
     the oracle's, the encoder the diagnostic reports the one expected."""
@@ -382,10 +381,6 @@ def test_staged_encoder_span_edge(variant, destw, staging):
                     cases.append((fmt, bpp, width, raw, skew))
     n = len(cases)
     b = capi.Batch(variant, n)
-    if staging == "mod_bulk0":
-        b.set_option("mod_bulk", 0)
-    elif staging == "tma0":
-        b.set_option("tma", 0)
     outs = [torch.zeros(48, 64, 4, dtype=torch.uint8, device="cuda") for _ in range(n)]
     h = 40
     keep, oras, imgs = [], [], []
@@ -416,10 +411,9 @@ def test_staged_encoder_span_edge(variant, destw, staging):
     torch.cuda.synchronize()
     paths = b.paths()
     for m, (fmt, bpp, width, raw, skew) in enumerate(cases):
-        assert bool(paths[m] & STAGED) == staged_ok(width, destw, bpp), (variant, staging, cases[m], paths[m])
+        assert bool(paths[m] & STAGED) == staged_ok(width, destw, bpp), (variant, cases[m], paths[m])
         got = b.signal(m, "analog")
-        assert np.array_equal(got, oras[m].analog), "%s %s %r: %s" % (variant, staging, cases[m],
-                                                                     S.diff_report("analog", got, oras[m].analog))
+        assert np.array_equal(got, oras[m].analog), "%s %r: %s" % (variant, cases[m], S.diff_report("analog", got, oras[m].analog))
     b.close()
 
 
@@ -443,13 +437,11 @@ def _store_cases(widths):
     return out
 
 
-def _check_store_cases(cases, staging):
+def _check_store_cases(cases):
     import torch
     from ntsc_crt_b200 import capi
     spec = layout.system_spec("pv1k")
     b = capi.Batch("pv1k", len(cases))
-    if staging == "mod_bulk0":
-        b.set_option("mod_bulk", 0)
     outs = [torch.zeros(8, 16, 4, dtype=torch.uint8, device="cuda") for _ in cases]
     oras, keep, residues = [], [], set()
     for m, (w, xoff) in enumerate(cases):
@@ -475,16 +467,14 @@ def _check_store_cases(cases, staging):
     for m in range(len(cases)):
         assert paths[m] & STAGED, (cases[m], paths[m])
         got = b.signal(m, "analog")
-        assert np.array_equal(got, oras[m].analog), "pv1k %s %r: %s" % (staging, cases[m],
-                                                                       S.diff_report("analog", got, oras[m].analog))
+        assert np.array_equal(got, oras[m].analog), "pv1k %r: %s" % (cases[m], S.diff_report("analog", got, oras[m].analog))
     b.close()
 
 
-@pytest.mark.parametrize("staging", ["default", "mod_bulk0"])
-def test_pv1k_staged_encoder_stores_at_every_line_phase(staging):
+def test_pv1k_staged_encoder_stores_at_every_line_phase():
     """raw pictures 1-4 samples wide (one word cut at both ends), 31-33, 63-65, and several chunks with every tail length
     mod 4, each at all 32 phases of the line start against the 32-byte sectors of analog[], xo even and odd"""
-    _check_store_cases(_store_cases(STORE_WIDTHS), staging)
+    _check_store_cases(_store_cases(STORE_WIDTHS))
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -106,17 +106,15 @@ def test_generic_monitor_inside_a_pair():
          per_monitor_knobs={1: dict(saturation=400, brightness=5000)})
 
 
-def test_generic_everywhere_and_plain_loads():
+def test_generic_everywhere():
     _run("ntsc", 640, 480, n=2, fields=2, options=(("generic_eq", 1),), knobs=dict(blend=0, scanlines=1))
-    _run("ntsc", 640, 480, n=2, fields=2, options=(("tma", 0),), knobs=dict(blend=1, scanlines=0))
 
 
-@pytest.mark.parametrize("mode", [1, 2])
-def test_both_asynchronous_staging_modes(mode):
-    """the signal windows reach shared memory by one bulk copy (TMA) per lane and stage, or by three 16-byte cp.async per
-    lane and stage (option "lines2_stage" 1 / 2); odd byte phases of the windows come from the noise-driven hsync"""
-    _run("ntsc", 832, 624, n=3, fields=4, options=(("lines2_stage", mode),), knobs=dict(blend=1, scanlines=1), noise=9)
-    _run("ntsc", 640, 480, n=2, fields=2, options=(("lines2_stage", mode),), knobs=dict(blend=0, scanlines=1), noise=0)
+def test_signal_windows_at_odd_byte_phases():
+    """the signal windows reach shared memory by three 16-byte cp.async per lane and stage from the 16-byte aligned address
+    below them; odd byte phases of the windows come from the noise-driven hsync"""
+    _run("ntsc", 832, 624, n=3, fields=4, knobs=dict(blend=1, scanlines=1), noise=9)
+    _run("ntsc", 640, 480, n=2, fields=2, knobs=dict(blend=0, scanlines=1), noise=0)
 
 
 def test_scanline_window():

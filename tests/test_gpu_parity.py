@@ -292,31 +292,6 @@ def test_dropin_vhs(color):
         S.assert_same_state(gpu.state(), ora.state(), "vhs demod %d" % it)
 
 
-def test_tma_and_plain_staging_agree():
-    """The TMA (cp.async.bulk) staging of the line kernel against plain loads, same kernel."""
-    import torch
-    from ntsc_crt_b200 import capi
-    img = torch.from_numpy(S.rand_image(832, 624, seed=11)).cuda()
-    outs = []
-    for tma in (1, 0):
-        b = capi.Batch("ntsc", 2)
-        b.set_option("tma", tma)
-        o = [torch.zeros(624, 832, 4, dtype=torch.uint8, device="cuda") for _ in range(2)]
-        for i in range(2):
-            b.set_monitor(i, o[i], noise=7 * i, blend=1, scanlines=1)
-            b.set_source(i, img, format=layout.PIX_BGRA, as_color=1, field=i, frame=0)
-        b.commit_monitors()
-        for _ in range(2):
-            b.modulate()
-            b.demodulate()
-        torch.cuda.synchronize()
-        outs.append([x.cpu().numpy() for x in o])
-        b.close()
-    for i in range(2):
-        assert np.array_equal(outs[0][i], outs[1][i])
-    assert outs[0][0].any()
-
-
 def test_batch_matches_independent_oracles():
     """crtx batch of 5 monitors with different knobs / noise = 5 independent reference instances."""
     import torch

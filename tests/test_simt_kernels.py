@@ -169,7 +169,7 @@ def test_other_thread_schedules(schedule):
     GPU would expose as a race, fails here."""
     import subprocess
     env = dict(os.environ, SIMT_SCHEDULE=schedule)
-    sel = "bloom_batch or pv1k_batch or template_batch or wire_ppm or wire_fade or tma_and_plain or fullsize"
+    sel = "bloom_batch or pv1k_batch or template_batch or wire_ppm or wire_fade or parity_batch_matches_independent_oracles or fullsize"
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-x", "-q", "-k", sel, "-p", "no:cacheprovider"],
                        env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, cwd=S.ROOT)
     assert r.returncode == 0, r.stdout[-3000:]
