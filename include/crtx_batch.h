@@ -29,25 +29,38 @@ typedef struct crtx_ctx crtx_ctx;
 
 /* the caller-settable part of struct CRT, plus crt_demodulate's `noise` argument */
 typedef struct crtx_monitor {
-    void *out; /* DEVICE image, outw * outh * bpp bytes */
+    void *out; /* DEVICE image: outh rows of outw * bpp bytes, out_pitch bytes apart */
     int outw, outh, out_format;
     int hue, brightness, contrast, saturation;
     int black_point, white_point;
     int scanlines, blend;
     unsigned v_fac;
     int noise;
+    int out_pitch; /* bytes between the starts of two output rows; 0 = dense (outw * bpp) */
 } crtx_monitor;
 
 /* struct NTSC_SETTINGS with the image on the DEVICE; fields a system lacks are ignored */
 typedef struct crtx_source {
-    const void *data; /* RGB systems: w*h*bpp bytes; NES: w*h unsigned short */
+    const void *data; /* h rows, pitch bytes apart; RGB systems: w*bpp bytes per row; NES: w unsigned short */
     int format, w, h;
     int raw, as_color, field, frame;
     int hue, xoffset, yoffset;
     int do_aberration;    /* CRT_SYSTEM_NTSCVHS */
     int dot_crawl_offset; /* CRT_SYSTEM_NES, _NESRGB, _SNES, _TEMP, _PV1K */
     int reinit;           /* CRT_SYSTEM_NES: settings.field_initialized was 0 */
+    int pitch;            /* bytes between the starts of two source rows; 0 = dense (w * bpp, NES w * 2) */
 } crtx_source;
+
+/* Row pitches.  A pitch of 0 means dense rows, which is what a zeroed struct gives.  Otherwise the pitch must be at
+ * least the row's bytes (outw * bpp, w * bpp, NES w * 2) and positive; 4-byte pixel formats need a pitch that is a
+ * multiple of 4 (as they need a 4-byte aligned image), NES sources an even one.  crtx_set_monitors, crtx_modulate and
+ * crtx_frames_host reject anything else, name the monitor and the rule in crtx_last_error(), and leave the context as it
+ * was.  No kernel writes a byte between the end of one row and the start of the next, so an image can be a window of a
+ * larger buffer (a cudaMallocPitch allocation, a decoder surface, one tile of a mosaic).  The fast paths need rows that
+ * start on 16-byte boundaries -- the image's address AND its pitch multiples of 16; other pitches take the general
+ * paths, with the same results.  Only the crtx_modulate / crtx_demodulate / crtx_frames_host images have pitches:
+ * the BMP / PPM wire kernels and crtx_fade_phosphors below work on dense arrays, whose layout the file formats and a
+ * pixel count fix. */
 
 /* the persistent decoder state of struct CRT */
 typedef struct crtx_state {
@@ -98,11 +111,14 @@ int crtx_demodulate(crtx_ctx *ctx, int first, int count, void *stream);
 
 /* host-buffer entry point: src[i].data and out_host[i] are HOST pointers; moves the images in, runs modulate +
  * demodulate, moves the decoded images out, all on `stream`; the monitors' `out` must have been set to device images
- * of the right size.  out_host[i] is the monitor's PERSISTENT host image, like the `out` buffer of the reference's
- * struct CRT: with page-locked (crtx_host_alloc / cudaHostAlloc) images whose rows are multiples of 16 bytes, only the
- * source rows the field reads (crt_ntsc.c:258-266) and only the output rows it writes (crt_core.c:428-432, 662-664)
- * cross PCIe, and every other row of out_host[i] keeps its bytes.  Pageable or odd-sized images, and option
- * "host_rows" 0, take whole-image copies. */
+ * of the right size.  The host images have the same pitches as the device ones: src[i].pitch for src[i].data, the
+ * monitor's out_pitch for out_host[i] (and for its `out`).  out_host[i] is the monitor's PERSISTENT host image, like
+ * the `out` buffer of the reference's struct CRT: with page-locked (crtx_host_alloc / cudaHostAlloc) images whose rows
+ * start on 16-byte boundaries (address and pitch multiples of 16; a dense image whose rows are not a multiple of 16
+ * bytes can get there by padding its rows), only the source rows the field reads (crt_ntsc.c:258-266) and only the
+ * output rows it writes (crt_core.c:428-432, 662-664) cross PCIe, and every other row of out_host[i], and the padding
+ * behind every row, keeps its bytes.  Pageable or unaligned images, and option "host_rows" 0, take whole-image copies
+ * (of the rows' bytes only). */
 int crtx_frames_host(crtx_ctx *ctx, int first, int count, const crtx_source *src,
                      void *const *out_host, void *stream);
 
@@ -148,14 +164,18 @@ int crtx_get_timing(crtx_ctx *ctx, float *ms /* [CRTX_NUM_KERNELS] */, long *lau
 int crtx_get_lines(crtx_ctx *ctx, int i, crtx_line *table /* crtx_lines() entries */, void *stream);
 long crtx_launch_count(crtx_ctx *ctx); /* kernels launched through this context so far */
 long crtx_lines2_count(crtx_ctx *ctx); /* of those, line passes taken by k_lines2 (two monitors per CTA, tabulated resampler: the
-                                         * stock IIR decoder on 4-byte pixels, 16-byte aligned images, outw a multiple of 4 in about
+                                         * stock IIR decoder on 4-byte pixels, 16-byte aligned rows, outw a multiple of 4 in about
                                          * [528, 1312]); every other geometry runs k_lines.  For tests and A/B runs (option "lines2"). */
 /* which code paths monitors [first, first + count) took: paths[i] has CRTX_PATH_GENERIC_EQ set when the last demodulate's sync
  * pass put monitor first + i on the wrap-exact equaliser (its carrier or brightness is outside the fast equaliser's exact range,
  * or option "generic_eq" is on), and CRTX_PATH_STAGED_MOD when the last modulate encoded its picture with the staged encoder
- * (the source span of a 32-sample chunk fits a stage row) rather than the gather encoder.  Synchronises `stream`. */
+ * (the source span of a 32-sample chunk fits a stage row) rather than the gather encoder, and CRTX_PATH_ROW16 when the line
+ * pass writes its output rows with 16-byte stores (k_lines2, or the row path of k_lines / k_lines_fir: 4-byte pixels, outw a
+ * multiple of 4, the image's address and out_pitch multiples of 16; never in the bloom build) rather than pixel by pixel.
+ * Synchronises `stream`. */
 #define CRTX_PATH_GENERIC_EQ 1
 #define CRTX_PATH_STAGED_MOD 2
+#define CRTX_PATH_ROW16 4
 int crtx_get_paths(crtx_ctx *ctx, int first, int count, int *paths, void *stream);
 /* options: "generic_eq", "timing", "mod_staged", "lines2", "host_rows" (0/1 switches), "host_src" (1:
  * crtx_frames_host lets the encoder read page-locked source images in place instead of copying them), and

@@ -25,14 +25,15 @@ class Monitor(C.Structure):  # crtx_monitor
     _fields_ = [("out", C.c_void_p), ("outw", C.c_int), ("outh", C.c_int), ("out_format", C.c_int),
                 ("hue", C.c_int), ("brightness", C.c_int), ("contrast", C.c_int),
                 ("saturation", C.c_int), ("black_point", C.c_int), ("white_point", C.c_int),
-                ("scanlines", C.c_int), ("blend", C.c_int), ("v_fac", C.c_uint), ("noise", C.c_int)]
+                ("scanlines", C.c_int), ("blend", C.c_int), ("v_fac", C.c_uint), ("noise", C.c_int),
+                ("out_pitch", C.c_int)]
 
 
 class Source(C.Structure):  # crtx_source
     _fields_ = [("data", C.c_void_p), ("format", C.c_int), ("w", C.c_int), ("h", C.c_int),
                 ("raw", C.c_int), ("as_color", C.c_int), ("field", C.c_int), ("frame", C.c_int),
                 ("hue", C.c_int), ("xoffset", C.c_int), ("yoffset", C.c_int),
-                ("do_aberration", C.c_int), ("dot_crawl_offset", C.c_int), ("reinit", C.c_int)]
+                ("do_aberration", C.c_int), ("dot_crawl_offset", C.c_int), ("reinit", C.c_int), ("pitch", C.c_int)]
 
 
 def source_table(sources):
@@ -42,6 +43,21 @@ def source_table(sources):
     dt = np.dtype([(n, "u8" if t is C.c_void_p else "i4") for n, t in Source._fields_], align=True)
     assert dt.itemsize == C.sizeof(Source), (dt.itemsize, C.sizeof(Source))
     return np.frombuffer(sources, dtype=dt)
+
+
+def row_pitch(t):
+    """Bytes between the starts of two rows of an image tensor: (h, w, bpp) bytes, or (h, w) 2-byte NES pixels.  The
+    rows may sit anywhere in a larger buffer (a column view of a mosaic, a crop), but each row's pixels must be packed:
+    anything else raises ValueError rather than letting a kernel write at the wrong offsets."""
+    if t.dim() == 3:
+        packed = t.stride(1) == t.shape[2] and t.stride(2) == 1
+    elif t.dim() == 2:
+        packed = t.stride(1) == 1
+    else:
+        raise ValueError("an image tensor is (h, w, bpp) or (h, w), not %s" % (tuple(t.shape),))
+    if not packed:
+        raise ValueError("image rows must hold packed pixels, got strides %s for shape %s" % (t.stride(), tuple(t.shape)))
+    return t.stride(0) * t.element_size()
 
 
 class State(C.Structure):  # crtx_state
@@ -144,10 +160,13 @@ class Batch:
         self._check(self.lib.crtx_set_option(self._ctx, name.encode(), int(value)))
 
     def set_monitor(self, i, out, fmt=layout.PIX_BGRA, noise=0, **knobs):
-        """out: torch uint8 CUDA tensor (outh, outw, bpp); knobs default to crt_reset's."""
+        """out: torch uint8 CUDA tensor (outh, outw, bpp) whose rows may be strided (row_pitch); knobs default to
+        crt_reset's."""
+        pitch = row_pitch(out)
         m = self.monitors[i]
         m.out = out.data_ptr()
         m.outh, m.outw = out.shape[0], out.shape[1]
+        m.out_pitch = pitch
         m.out_format = fmt
         m.hue, m.brightness, m.contrast, m.saturation = 0, 0, 180, 10
         m.black_point, m.white_point, m.scanlines, m.blend, m.v_fac = 0, 100, 0, 0, 0
@@ -163,10 +182,13 @@ class Batch:
                                                       C.POINTER(Monitor))))
 
     def set_source(self, i, img, **settings):
-        """img: torch CUDA tensor (h, w, bpp) uint8, or (h, w) int16/uint16 for the NES."""
+        """img: torch CUDA tensor (h, w, bpp) uint8, or (h, w) int16/uint16 for the NES, whose rows may be strided
+        (row_pitch)."""
+        pitch = row_pitch(img)
         s = self.sources[i]
         s.data = img.data_ptr()
         s.h, s.w = img.shape[0], img.shape[1]
+        s.pitch = pitch
         for k, v in settings.items():
             setattr(s, k, v)
         self._keep[("src", i)] = img
@@ -209,6 +231,7 @@ class Batch:
 
     PATH_GENERIC_EQ = 1  # CRTX_PATH_GENERIC_EQ: the last demodulate decoded the monitor with the wrap-exact equaliser
     PATH_STAGED_MOD = 2  # CRTX_PATH_STAGED_MOD: the last modulate encoded its picture with the staged encoder
+    PATH_ROW16 = 4  # CRTX_PATH_ROW16: the line pass writes the monitor's rows with 16-byte stores (16-byte aligned rows)
 
     def paths(self, first=0, count=None, stream=0):
         """crtx_get_paths: per monitor, the PATH_* bits of the code paths its last modulate and demodulate took"""

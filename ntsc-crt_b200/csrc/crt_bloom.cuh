@@ -146,7 +146,7 @@ __global__ void __launch_bounds__(kBloomWarps * 32) k_lines_bloom(const MonCfg *
     __syncwarp();
 
     // ---- pixels (crt_core.c:551-664)
-    const int bpp = geo.bpp, pitch = geo.outw * bpp;
+    const int bpp = geo.bpp, pitch = geo.pitch;
     int rp, gp, bp;
     fmt_positions(geo.out_format, rp, gp, bp);
     const int ap = (bpp == 4) ? (6 - rp - gp - bp) : -1; // the remaining byte of a 4-byte pixel

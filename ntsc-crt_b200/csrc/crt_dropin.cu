@@ -254,6 +254,7 @@ void crt_modulate(struct CRT *v, struct NTSC_SETTINGS *s)
 #endif
     const size_t img_bytes = (size_t) s->w * s->h * bpp;
 #endif
+    src.pitch = (int) src_row_bytes(src.format, src.w); // the reference's images are dense
     ensure(&sh->d_img, &sh->img_bytes, img_bytes ? img_bytes : 4, sh->stream);
     cuda_or_die(cudaMemcpyAsync(sh->d_img, s->data, img_bytes, cudaMemcpyHostToDevice, sh->stream), "image upload");
     src.data = sh->d_img;

@@ -40,6 +40,8 @@ __device__ __forceinline__ int wadd(int a, int b) { return (int) ((unsigned) a +
 __device__ __forceinline__ int wsub(int a, int b) { return (int) ((unsigned) a - (unsigned) b); }
 __device__ __forceinline__ int posmod(int x, int n) { return ((x % n) + n) % n; }
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return min(max(v, lo), hi); }
+// byte offset of image row `row` (>= 0) at `pitch` (> 0) bytes per row: 64-bit, one 32 x 32 -> 64 multiplication
+__device__ __forceinline__ size_t row_offset(int row, int pitch) { return (size_t) (unsigned) row * (unsigned) pitch; }
 
 __device__ __forceinline__ int quarter_d(int a)
 {
@@ -240,7 +242,8 @@ __device__ __forceinline__ void load_rgb(const unsigned char *data, size_t pix, 
 __host__ __device__ __forceinline__ bool mod_staged_ok(const SrcCfg &s, int destw);
 template <bool STAGED> __host__ __device__ __forceinline__ bool mod_takes(const SrcCfg &s);
 
-__global__ void __launch_bounds__(256) k_mod_picture_rgb(const SrcCfg *__restrict__ srcs,
+// (256, 2): its shared memory fits two CTAs per SM; a higher target spills the 64-bit row addresses
+__global__ void __launch_bounds__(256, 2) k_mod_picture_rgb(const SrcCfg *__restrict__ srcs,
                                                          const MonCfg *__restrict__ cfgs,
                                                          signed char *__restrict__ analog_base, int first,
                                                          int skip_staged)
@@ -274,7 +277,7 @@ __global__ void __launch_bounds__(256) k_mod_picture_rgb(const SrcCfg *__restric
     int rp, gp, bp;
     fmt_positions(s.format, rp, gp, bp);
     const unsigned char *data = static_cast<const unsigned char *>(s.data);
-    const bool aligned4 = ((reinterpret_cast<uintptr_t>(data) & 3) == 0);
+    const bool aligned4 = (((reinterpret_cast<uintptr_t>(data) | (uintptr_t) s.pitch) & 3) == 0);
 
     // five carrier phases (PV-1000): the phase of a sample is not a compile-time constant of the 4-sample inner
     // step, so the tables live in shared memory, [I | Q][colour row][phase]
@@ -306,7 +309,6 @@ __global__ void __launch_bounds__(256) k_mod_picture_rgb(const SrcCfg *__restric
     int row = (int) (((long long) min(y, desth - 1) * s.h) / desth) + (field * s.h + desth) / desth / 2;
     if (row >= s.h) row = s.h - 1;
     if (s.compact) row = min(y, desth - 1); // crtx_frames_host staged exactly those rows, in line order (k_rows_gather)
-    const int rowoff = row * s.w;
 
     int hy = 0, hi = 0, hq = 0;
     for (int c0 = 0; c0 < destw; c0 += kModChunk) {
@@ -316,11 +318,11 @@ __global__ void __launch_bounds__(256) k_mod_picture_rgb(const SrcCfg *__restric
         const int cola = (int) (((long long) min(xa, destw - 1) * s.w) / destw);
         const int colb = (int) (((long long) min(xb, destw - 1) * s.w) / destw);
         for (int l = 0; l < nlines; l++) {
-            const int ro = __shfl_sync(0xffffffffu, rowoff, l);
+            const unsigned char *rowp = data + row_offset(__shfl_sync(0xffffffffu, row, l), s.pitch);
 #pragma unroll
             for (int half = 0; half < 2; half++) {
                 int r, g, b;
-                load_rgb(data, (size_t) ro + (half ? colb : cola), bpp, rp, gp, bp, aligned4, r, g, b);
+                load_rgb(rowp, half ? colb : cola, bpp, rp, gp, bp, aligned4, r, g, b);
                 int fy = (19595 * r + 38470 * g + 7471 * b) >> 14; // crt_ntsc.c:308-310
                 int fi = (39059 * r - 18022 * g - 21103 * b) >> 14;
                 int fq = (13894 * r - 34275 * g + 20382 * b) >> 14;
@@ -381,7 +383,8 @@ __global__ void __launch_bounds__(256) k_mod_picture_rgb(const SrcCfg *__restric
 // Usable when the chunk's source span fits a stage row; other monitors return at once and are
 // handled by k_mod_picture_rgb (gather variant), which in turn skips the ones done here.
 // The source image must be readable up to the next 16-byte boundary past its last pixel
-// (true of any cudaMalloc / torch allocation; include/crtx_batch.h).
+// (true of any cudaMalloc / torch allocation; include/crtx_batch.h).  A row's copy covers the 16-byte aligned superset
+// of its span, which may take in bytes of the padding between rows: they land in the stage and are never used.
 // ---------------------------------------------------------------------------------------
 constexpr int kModSChunk = 32;                     // samples per chunk
 constexpr int kModSSpan = 192;                     // largest staged span the kernel accepts (incl. alignment slack)
@@ -403,8 +406,9 @@ __host__ __device__ __forceinline__ bool mod_staged_ok(const SrcCfg &s, int dest
     if (bpp == 0 || destw <= 0 || s.w <= 0 || (kCc != 4 && kCc != 5)) return false; // (four or five samples per carrier period)
     // widest source span of a chunk: ceil(32 * w / destw) + 1 pixels, plus 15 bytes of alignment
     const long long span = ((long long) kModSChunk * s.w + destw - 1) / destw + 1;
+    // 4-byte pixels are read from the stage as words: every row must start on a 4-byte boundary
     return span * bpp + 15 + 16 <= kModSSpan && s.w <= 65535
-        && (bpp != 4 || (reinterpret_cast<uintptr_t>(s.data) & 3) == 0);
+        && (bpp != 4 || ((reinterpret_cast<uintptr_t>(s.data) | (uintptr_t) s.pitch) & 3) == 0);
 }
 
 template <bool STAGED>
@@ -552,7 +556,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
     int row = (int) (((long long) y * s.h) / desth) + (field * s.h + desth) / desth / 2;
     if (row >= s.h) row = s.h - 1;
     if (s.compact) row = y; // crtx_frames_host staged exactly those rows, in line order (k_rows_gather)
-    const unsigned char *rowp = data + (size_t) row * s.w * bpp;
+    const unsigned char *rowp = data + row_offset(row, s.pitch);
 
     // chunk c covers samples [32c, 32c + 32); its span of source columns f0..f1 is staged from the 16-byte aligned address
     // at or below pixel f0.  Returns the offset of pixel f0 from that address.
@@ -771,7 +775,7 @@ __global__ void __launch_bounds__(256) k_mod_nes(const SrcCfg *__restrict__ srcs
                 analog[n * kHres + t] = (signed char) ((t >= kSyncBeg && t < sync_end) ? kSync : kBlank);
         }
     }
-    const unsigned short *data = static_cast<const unsigned short *>(s.data);
+    const unsigned char *data = static_cast<const unsigned char *>(s.data);
     for (int y = part; y < kLines; y += kNesParts) {
         const int n = y + yo;
         // every byte of a picture line is written by this one CTA, in order: skeleton, burst, picture
@@ -788,7 +792,9 @@ __global__ void __launch_bounds__(256) k_mod_nes(const SrcCfg *__restrict__ srcs
         int row = (y * s.h) / kLines;
         if (row >= s.h) row = s.h - 1; // the reference reads one row past the image here (undefined)
         if (row < 0) row = 0;
-        const unsigned short *src_row = data + row * s.w;
+        // (the pitch is read per line: held in a register for the whole kernel it takes the kernel past 32 registers,
+        // and 8 CTAs per SM to 6)
+        const unsigned short *src_row = reinterpret_cast<const unsigned short *>(data + row_offset(row, __ldg(&srcs[m].pitch)));
         const int phase0 = ((y + yo + s.dot_crawl_offset) % 3) * 4;
         for (int x = tid; x < kAvLen; x += 256) { // crt_nes.c:180-193
             const int p = __ldg(src_row + (x * s.w) / kAvLen) & 0x1ff;
@@ -855,7 +861,7 @@ __global__ void __launch_bounds__(256) k_mod_snes(const SrcCfg *__restrict__ src
     int rp, gp, bp;
     fmt_positions(s.format, rp, gp, bp);
     const unsigned char *data = static_cast<const unsigned char *>(s.data);
-    const bool word_pixels = (bpp == 4) && ((reinterpret_cast<uintptr_t>(data) & 3) == 0);
+    const bool word_pixels = (bpp == 4) && (((reinterpret_cast<uintptr_t>(data) | (uintptr_t) s.pitch) & 3) == 0);
 
     for (int n = part; n < kVres; n += kSnesParts) {
         signed char *line = analog + n * kHres;
@@ -884,7 +890,7 @@ __global__ void __launch_bounds__(256) k_mod_snes(const SrcCfg *__restrict__ src
         if (xo < kAvBeg || n < kTop) __syncthreads(); // block-uniform condition
         int sy = (y * s.h) / desth;
         if (sy >= s.h) sy = s.h - 1; // (never taken for y < desth; the reference clamps to one row past the image)
-        const unsigned char *src_row = data + (size_t) sy * s.w * bpp;
+        const unsigned char *src_row = data + row_offset(sy, s.pitch);
         const int ph = n % kVper;
         constexpr int kPer = (kAvLen + 255) / 256; // samples per thread and line
         unsigned px[kPer];
@@ -926,7 +932,8 @@ __global__ void __launch_bounds__(256) k_mod_snes(const SrcCfg *__restrict__ src
 
 constexpr int kNesRgbParts = 8; // CTAs per monitor; CTA p owns signal lines n with n % kNesRgbParts == p
 
-__global__ void __launch_bounds__(256) k_mod_nesrgb(const SrcCfg *__restrict__ srcs, const MonCfg *__restrict__ cfgs,
+// (256, 8): the kernel fits 32 registers without spilling, and keeps 8 CTAs per SM
+__global__ void __launch_bounds__(256, 8) k_mod_nesrgb(const SrcCfg *__restrict__ srcs, const MonCfg *__restrict__ cfgs,
                                                     MonState *__restrict__ states, signed char *__restrict__ analog_base,
                                                     int first)
 {
@@ -958,7 +965,7 @@ __global__ void __launch_bounds__(256) k_mod_nesrgb(const SrcCfg *__restrict__ s
     int rp, gp, bp;
     fmt_positions(s.format, rp, gp, bp);
     const unsigned char *data = static_cast<const unsigned char *>(s.data);
-    const bool word_pixels = (bpp == 4) && ((reinterpret_cast<uintptr_t>(data) & 3) == 0);
+    const bool word_pixels = (bpp == 4) && (((reinterpret_cast<uintptr_t>(data) | (uintptr_t) s.pitch) & 3) == 0);
 
     for (int n = part; n < kVres; n += kNesRgbParts) {
         signed char *line = analog + n * kHres;
@@ -975,7 +982,7 @@ __global__ void __launch_bounds__(256) k_mod_nesrgb(const SrcCfg *__restrict__ s
         }
         int sy = (y * s.h) / kLines;
         if (sy >= s.h) sy = s.h - 1; // (never taken; the reference clamps to one row past the image)
-        const unsigned char *src_row = data + (size_t) sy * s.w * bpp;
+        const unsigned char *src_row = data + row_offset(sy, s.pitch);
         const int ph = n % kVper;
         constexpr int kPer = (kAvLen + 255) / 256;
         unsigned px[kPer];

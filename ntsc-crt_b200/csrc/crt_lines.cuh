@@ -141,18 +141,26 @@ constexpr int kMaxOutw = 8192;
 
 struct LinesGeom { // uniform over a launch: host groups monitors by these (crtx.cu)
     int outw, out_format, bpp, blend;
+    int pitch; // bytes between output rows (MonCfg::out_pitch, shared by every monitor of the launch)
     int pass; // -1: every line; -2: only the last line of each shared-row run; >= 0: lines at this run position
     int rnd; // 32768, passed as an argument so that it lives in a register (see pole())
     int dx;  // ((AV_LEN - 1) << 12) / outw (crt_core.c:527), computed by the host: no division in the kernels
     int line_lo, line_hi; // decoded lines [lo, hi) this launch may touch (scanline-block sharding across ranks)
 };
 
+// The 16-byte row path of k_lines and k_lines_fir (and a condition of k_lines2): 4-byte pixels, rows of whole 16-byte
+// groups that start on 16-byte boundaries (the image's address and its pitch multiples of 16).  crtx_get_paths reports it.
+__host__ __device__ inline bool rows16_ok(const void *out, int pitch, int outw, int bpp)
+{
+    return bpp == 4 && (outw & 3) == 0 && ((reinterpret_cast<uintptr_t>(out) | (uintptr_t) pitch) & 15) == 0;
+}
+
 // Write `cnt` (<= 16) finished pixels [k0, k0 + cnt) of every active line of this warp
 // (crt_core.c:584-664).  The tile holds 16 pixel columns per line; pixels are already in storage byte
 // order and, when blending, pre-halved with the alpha byte forced to 0xff, so the blend is
 // (old >> 1 & mask) + new on whole words.
 //
-// 128-bit path (4-byte pixels, 16-byte aligned rows): 4 lanes per row, 8 rows per pass, 4 passes.  Each
+// 128-bit path (4-byte pixels, rows that start on 16-byte boundaries: image address and pitch multiples of 16): 4 lanes per row, 8 rows per pass, 4 passes.  Each
 // lane keeps, for its 4 (row, quad) slots, the row pointer and the number of rows to write
 // (crt_core.c:662-664), and -- when blending -- the previous image's pixels of the NEXT 16-pixel block,
 // fetched right after this block is written so that the DRAM latency hides behind a whole sub-chunk
@@ -198,7 +206,7 @@ __device__ __forceinline__ void flush16_vec(const unsigned *tile, const RowSlots
 __device__ __forceinline__ void flush16_scalar(const unsigned *tile, const LinesGeom &geo, unsigned char *out, int k0,
                                                int cnt, int lane, int beg, int nrows, unsigned blend_mask)
 {
-    const int pitch = geo.outw * geo.bpp;
+    const int pitch = geo.pitch;
     int rp, gp, bp;
     fmt_positions(geo.out_format, rp, gp, bp);
     const int j = lane & 15;
@@ -282,11 +290,11 @@ k_lines(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, co
     unsigned char *out = cfg->out;
     const int beg = active ? rec.beg : -1;
     const int nrows = active ? max(1, rec.end - cfg->scanlines - rec.beg) : 0; // crt_core.c:662-664
-    const bool vec = (MODE != 2) && ((geo.outw & 3) == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
+    const bool vec = (MODE != 2) && rows16_ok(out, geo.pitch, geo.outw, 4);
     LinesGeom fgeo = geo; // what the scalar flush branches on, pinned to the template mode
     fgeo.bpp = (MODE == 2) ? 3 : 4;
     if (MODE != 2) fgeo.blend = (MODE == 1);
-    const int pitch = geo.outw * fgeo.bpp;
+    const int pitch = geo.pitch;
     RowSlots rs;
     uint4 oldv[4];
 #pragma unroll

@@ -57,7 +57,7 @@ __host__ __device__ constexpr int lines2_smem(int outw)
 }
 static_assert(lines2_smem(kL2MaxOutw) <= 227 * 1024, "k_lines2 shared memory");
 
-// the geometries k_lines2 takes (the rest of the conditions -- pixel size, alignment, fast equaliser -- are the caller's)
+// the geometries k_lines2 takes (the rest of the conditions -- pixel size, row alignment, fast equaliser -- are the caller's)
 __host__ __device__ inline bool lines2_geometry_ok(int outw)
 {
     if (kCc != 4 || outw < 16 || outw > kL2MaxOutw || (outw & 3)) return false;
@@ -160,7 +160,7 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
     unsigned char *out = cfg->out;
     const int beg = active ? rec.beg : -1;
     const int nrows = active ? max(1, rec.end - cfg->scanlines - rec.beg) : 0; // crt_core.c:662-664
-    const int pitch = geo.outw * 4;
+    const int pitch = geo.pitch;
     TileRows tr;
 #pragma unroll
     for (int it = 0; it < 4; it++) {

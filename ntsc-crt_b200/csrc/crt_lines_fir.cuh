@@ -160,10 +160,10 @@ k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states
     unsigned ph_sig = 0, ph_old = 0; // bit b: parity of the next wait on buffer b
 
     constexpr int bpp = (MODE == 2) ? 3 : 4;
-    const int pitch = geo.outw * bpp;
-    // rows go through shared memory and bulk copies when they are 16-byte granular; otherwise (3-byte
-    // pixels, odd widths, unaligned images) every lane reads and writes its own pixels
-    const bool bulk = (MODE != 2) && ((geo.outw & 3) == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
+    const int pitch = geo.pitch;
+    // rows go through shared memory and bulk copies when they are 16-byte granular and start on 16-byte boundaries;
+    // otherwise (3-byte pixels, odd widths, unaligned images or pitches) every lane reads and writes its own pixels
+    const bool bulk = (MODE != 2) && rows16_ok(out, pitch, geo.outw, 4);
     const bool prefetch_old = bulk && (MODE == 1);
     const signed char *inp = inp_base + (size_t) m * kSignalBytes;
     const unsigned dx = (unsigned) (((kAvLen - 1) << 12) / geo.outw); // crt_core.c:527

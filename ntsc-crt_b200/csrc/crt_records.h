@@ -17,6 +17,7 @@ struct MonCfg { // host -> device, the caller-settable part of struct CRT
     int scanlines, blend;
     unsigned v_fac;
     int noise;
+    int out_pitch; // bytes between output rows (never 0: the host resolves crtx_monitor's 0 to outw * bpp)
 };
 
 struct MonState { // device resident, the persistent decoder state of struct CRT
@@ -38,6 +39,7 @@ struct SrcCfg { // host -> device, struct NTSC_SETTINGS
     int dot_crawl_offset;
     int reinit;
     int compact; // internal (crtx_frames_host): `data` holds only the rows this field reads, picture line y in row y
+    int pitch;   // bytes between source rows (resolved by the host: crtx_source's 0 becomes w * bpp, NES w * 2)
 };
 
 typedef crtx_line LineRec; // 32 bytes

@@ -7,6 +7,7 @@
 // papered over.
 #include <cuda_runtime.h>
 
+#include <limits.h>
 #include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -105,12 +106,13 @@ static void launch_lines_mode(crtx_ctx *ctx, int count, int lo, const LinesGeom 
 }
 
 // k_lines2 (crt_lines2.cuh): two monitors per CTA, tabulated resampler.  Taken when the whole run qualifies: the stock
-// IIR decoder, 4-byte pixels, every line owning its rows, a width the pixel ring covers, 16-byte aligned images.
+// IIR decoder, 4-byte pixels, every line owning its rows, a width the pixel ring covers, rows that start on 16-byte
+// boundaries (the run's pitch and every image's address multiples of 16).
 #if CRTX_HAS_LINES2
 static bool lines2_eligible(const crtx_ctx *ctx, int count, int lo, const LinesGeom &geo)
 {
     if (!ctx->opt_lines2) return false;
-    if (geo.bpp != 4 || geo.pass != -1 || !lines2_geometry_ok(geo.outw)) return false;
+    if (geo.bpp != 4 || geo.pass != -1 || !lines2_geometry_ok(geo.outw) || (geo.pitch & 15)) return false;
     for (int i = lo; i < lo + count; i++)
         if (reinterpret_cast<uintptr_t>(ctx->h_cfg[i].out) & 15) return false;
     return true;
@@ -441,7 +443,8 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
         pre += 1;
     }
     // The line kernel takes the output geometry as launch-uniform arguments: split the range into
-    // runs of monitors that share it (normally one run).
+    // runs of monitors that share it (normally one run).  The row pitch is part of it: a batch of dense images, or of
+    // tiles of one mosaic, has one pitch, so it costs no launch and the kernels read it from their parameters.
     int launched = 0;
     for (int lo = first; lo < first + count;) {
         const MonCfg &c0 = ctx->h_cfg[lo];
@@ -449,7 +452,7 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
         while (hi < first + count) {
             const MonCfg &c = ctx->h_cfg[hi];
             if (c.outw != c0.outw || c.out_format != c0.out_format || c.blend != c0.blend || c.outh != c0.outh
-                || c.v_fac != c0.v_fac)
+                || c.v_fac != c0.v_fac || c.out_pitch != c0.out_pitch)
                 break;
             hi++;
         }
@@ -457,6 +460,7 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
         geo.outw = c0.outw;
         geo.out_format = c0.out_format;
         geo.bpp = c0.bpp;
+        geo.pitch = c0.out_pitch;
         geo.blend = c0.blend ? 1 : 0;
         geo.rnd = 32768;
         geo.dx = c0.outw > 0 ? ((kAvLen - 1) << 12) / c0.outw : 0;
@@ -623,12 +627,16 @@ __global__ void k_fade_phosphors(unsigned *__restrict__ image, size_t npix)
 //   k_rows_gather   host image -> the monitor's staging slot, picture line y in row y (SrcCfg::compact)
 //   k_rows_scatter  device image -> host image, the rows the line table says this field wrote; every other row
 //                   of the host image keeps its content, exactly as the reference's own `out` buffer does.
-// Pageable, unmapped or unaligned host buffers take the whole-image cudaMemcpyAsync as before.
+// Both need rows that start on 16-byte boundaries (image address and pitch multiples of 16).  The gather reads each
+// source row's 16-byte aligned superset into slot rows that far apart; the scatter writes exactly a row's bytes, so
+// the padding between the host image's rows keeps its content too.  Pageable, unmapped or unaligned host buffers take
+// whole-image copies.
 // ---------------------------------------------------------------------------------------------------------
 struct RowGather {
     const unsigned char *src; // device mapping of the page-locked host image, or NULL: not a row job
     unsigned char *dst;       // staging slot
-    int row_bytes, h, desth, field;
+    int row_bytes;            // bytes copied per row, and the slot's pitch: the source row's bytes rounded up to 16
+    int src_pitch, h, desth, field;
 };
 
 constexpr int kRowWarps = 8;
@@ -654,7 +662,7 @@ __global__ void __launch_bounds__(kRowWarps * 32) k_rows_gather(const RowGather 
     if (!j.src || y >= j.desth) return;
     int row = (int) (((long long) y * j.h) / j.desth) + (j.field * j.h + j.desth) / j.desth / 2; // crt_ntsc.c:258-266
     if (row >= j.h) row = j.h - 1; // (as the encoder kernels: the reference's one-row over-read is not reproduced)
-    copy_row16(reinterpret_cast<const uint4 *>(j.src + (size_t) row * j.row_bytes),
+    copy_row16(reinterpret_cast<const uint4 *>(j.src + (size_t) row * j.src_pitch),
                reinterpret_cast<uint4 *>(j.dst + (size_t) y * j.row_bytes), j.row_bytes / 16, lane);
 }
 
@@ -670,11 +678,12 @@ k_rows_scatter(const MonCfg *__restrict__ cfgs, const LineRec *__restrict__ line
     const LineRec rec = lines[(size_t) m * kLines + k];
     if (rec.beg < 0) return;
     const MonCfg cfg = cfgs[m];
-    const int pitch = cfg.outw * cfg.bpp;
+    const int row_bytes = cfg.outw * cfg.bpp;
     const int nrows = max(1, rec.end - cfg.scanlines - rec.beg); // crt_core.c:662-664
     for (int r = 0; r < nrows; r++) {
-        const size_t off = (size_t) (rec.beg + r) * pitch;
-        copy_row16(reinterpret_cast<const uint4 *>(cfg.out + off), reinterpret_cast<uint4 *>(host + off), pitch / 16, lane);
+        const size_t off = (size_t) (rec.beg + r) * cfg.out_pitch;
+        copy_row16(reinterpret_cast<const uint4 *>(cfg.out + off), reinterpret_cast<uint4 *>(host + off), row_bytes / 16, lane);
+        if (lane < (row_bytes & 15)) host[off + (row_bytes & ~15) + lane] = cfg.out[off + (row_bytes & ~15) + lane]; // (pitched rows)
     }
 }
 
@@ -704,9 +713,27 @@ void fill_src(SrcCfg *d, const crtx_source *s)
     d->aberration = 0;
     d->dot_crawl_offset = s->dot_crawl_offset;
     d->reinit = s->reinit;
+    d->pitch = s->pitch ? s->pitch : (int) src_row_bytes(s->format, s->w); // (check_sources: fits an int)
 #if (CRT_SYSTEM == CRT_SYSTEM_NES)
     d->format = CRT_PIX_FORMAT_RGB; // unused by the NES encoder
 #endif
+}
+
+// crtx_modulate / crtx_frames_host: the source pitches, all of them before anything is applied
+static int check_sources(int first, int count, const crtx_source *src)
+{
+    for (int i = 0; i < count; i++) {
+        const long long row = src_row_bytes(src[i].format, src[i].w);
+        const int p = src[i].pitch;
+        if (p < 0) return fail("monitor %d: negative source pitch %d", first + i, p);
+        if (p == 0 && row > INT_MAX) return fail("monitor %d: source rows of %lld bytes need a pitch above INT_MAX", first + i, row);
+        if (p == 0) continue;
+        if (p < row) return fail("monitor %d: source pitch %d below the row's %lld bytes", first + i, p, row);
+        if (kIsNes && (p & 1)) return fail("monitor %d: source pitch %d is odd, NES rows hold 2-byte pixels", first + i, p);
+        if (!kIsNes && bpp_of(src[i].format) == 4 && (p & 3))
+            return fail("monitor %d: source pitch %d is not a multiple of 4, which 4-byte pixel formats need", first + i, p);
+    }
+    return 0;
 }
 
 } // namespace crt
@@ -857,8 +884,14 @@ int crtx_set_monitors(crtx_ctx *ctx, int first, int count, const crtx_monitor *m
             return fail("monitor %d: negative output size %d x %d", first + i, m[i].outw, m[i].outh);
         if (m[i].outw > kMaxOutw)
             return fail("monitor %d: outw %d above the supported maximum %d", first + i, m[i].outw, kMaxOutw);
-        if (bpp_of(m[i].out_format) == 4 && (reinterpret_cast<uintptr_t>(m[i].out) & 3))
+        const int bpp = bpp_of(m[i].out_format);
+        if (bpp == 4 && (reinterpret_cast<uintptr_t>(m[i].out) & 3))
             return fail("monitor %d: 4-byte pixel formats need a 4-byte aligned device image", first + i);
+        if (m[i].out_pitch < 0) return fail("monitor %d: negative output pitch %d", first + i, m[i].out_pitch);
+        if (m[i].out_pitch != 0 && m[i].out_pitch < m[i].outw * bpp)
+            return fail("monitor %d: output pitch %d below the row's %d bytes", first + i, m[i].out_pitch, m[i].outw * bpp);
+        if (bpp == 4 && (m[i].out_pitch & 3))
+            return fail("monitor %d: output pitch %d is not a multiple of 4, which 4-byte pixel formats need", first + i, m[i].out_pitch);
     }
     // only what really changed travels to the device (the drop-in calls re-send every knob before every call)
     int lo = ctx->n, hi = 0, tlo = ctx->n, thi = 0;
@@ -880,6 +913,7 @@ int crtx_set_monitors(crtx_ctx *ctx, int first, int count, const crtx_monitor *m
         c.blend = m[i].blend;
         c.v_fac = m[i].v_fac;
         c.noise = m[i].noise;
+        c.out_pitch = m[i].out_pitch ? m[i].out_pitch : c.outw * c.bpp;
         MonCfg &old = ctx->h_cfg[first + i];
         if (memcmp(&c, &old, sizeof(MonCfg)) == 0) continue;
         if (c.outw != old.outw || c.outh != old.outh || c.out_format != old.out_format) {
@@ -1009,6 +1043,7 @@ static int modulate_sources(crtx_ctx *ctx, int first, int count, const crtx_sour
 
 int crtx_modulate(crtx_ctx *ctx, int first, int count, const crtx_source *src, void *stream)
 {
+    if (check_range(ctx, first, count) || check_sources(first, count, src)) return 1;
     return modulate_sources(ctx, first, count, src, NULL, stream);
 }
 
@@ -1019,12 +1054,15 @@ int crtx_demodulate(crtx_ctx *ctx, int first, int count, void *stream)
 
 int crtx_frames_host(crtx_ctx *ctx, int first, int count, const crtx_source *src, void *const *out_host, void *stream)
 {
-    if (check_range(ctx, first, count)) return 1;
+    if (check_range(ctx, first, count) || check_sources(first, count, src)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // device staging for the source images, one slot per monitor
+    // device staging for the source images, one slot per monitor: the whole image with dense rows, or the rows a field
+    // reads (up to kDestH of them, whatever the image's height) at the row's bytes rounded up to 16
     size_t need = 0;
     for (int i = 0; i < count; i++) {
-        size_t b = (size_t) src[i].w * src[i].h * (kIsNes ? 2 : bpp_of(src[i].format));
+        const long long row = src_row_bytes(src[i].format, src[i].w);
+        size_t b = (size_t) (row * src[i].h);
+        if (row > 0 && (size_t) ((row + 15) & ~15LL) * kDestH > b) b = (size_t) ((row + 15) & ~15LL) * kDestH;
         b = (b + 255) & ~(size_t) 255;
         if (b > need) need = b;
     }
@@ -1041,7 +1079,8 @@ int crtx_frames_host(crtx_ctx *ctx, int first, int count, const crtx_source *src
     std::vector<RowGather> jobs(count);
     int row_jobs = 0, max_desth = 0;
     for (int i = 0; i < count; i++) {
-        size_t b = (size_t) src[i].w * src[i].h * (kIsNes ? 2 : bpp_of(src[i].format));
+        const long long row_bytes = src_row_bytes(src[i].format, src[i].w);
+        const int pitch = src[i].pitch ? src[i].pitch : (int) row_bytes;
         jobs[i].src = NULL;
         if (ctx->opt_host_src) {
             // "host_src": the encoder reads a page-locked source image in place over PCIe (A/B switch; the encoder's
@@ -1054,14 +1093,16 @@ int crtx_frames_host(crtx_ctx *ctx, int first, int count, const crtx_source *src
         }
         unsigned char *slot = ctx->d_src_img + ctx->src_slot * (size_t) (first + i);
         dev[i].data = slot;
+        dev[i].pitch = 0; // a whole image lands in its slot with dense rows
 #if CRT_B200_BANDLIMITED
-        const int row_bytes = src[i].w * bpp_of(src[i].format);
-        void *map = (ctx->opt_host_rows && row_bytes > 0 && (row_bytes & 15) == 0 && src[i].h > 0) ? host_mapping(src[i].data) : NULL;
+        void *map = (ctx->opt_host_rows && row_bytes > 0 && (pitch & 15) == 0 && src[i].h > 0) ? host_mapping(src[i].data) : NULL;
         if (map && (reinterpret_cast<uintptr_t>(map) & 15) == 0) {
             RowGather &j = jobs[i];
             j.src = static_cast<const unsigned char *>(map);
             j.dst = slot;
-            j.row_bytes = row_bytes;
+            j.row_bytes = (int) ((row_bytes + 15) & ~15LL); // (<= pitch)
+            j.src_pitch = pitch;
+            dev[i].pitch = j.row_bytes;
             j.h = src[i].h;
             j.desth = src[i].raw ? (src[i].h < kDestH ? src[i].h : kDestH) : kDestH; // crt_ntsc.c:132-133, 163-172
             j.field = src[i].field & 1;
@@ -1071,7 +1112,11 @@ int crtx_frames_host(crtx_ctx *ctx, int first, int count, const crtx_source *src
             continue;
         }
 #endif
-        CUDA_TRY(cudaMemcpyAsync(slot, src[i].data, b, cudaMemcpyHostToDevice, st));
+        if (pitch == row_bytes)
+            CUDA_TRY(cudaMemcpyAsync(slot, src[i].data, (size_t) (row_bytes * src[i].h), cudaMemcpyHostToDevice, st));
+        else if (src[i].h > 0)
+            CUDA_TRY(cudaMemcpy2DAsync(slot, (size_t) row_bytes, src[i].data, (size_t) pitch, (size_t) row_bytes, (size_t) src[i].h,
+                                       cudaMemcpyHostToDevice, st));
     }
     if (row_jobs) {
         CUDA_TRY(cudaMemcpyAsync(static_cast<RowGather *>(ctx->d_row_jobs) + first, jobs.data(), sizeof(RowGather) * count, cudaMemcpyHostToDevice, st));
@@ -1086,8 +1131,8 @@ int crtx_frames_host(crtx_ctx *ctx, int first, int count, const crtx_source *src
     for (int i = 0; i < count; i++) {
         const MonCfg &c = ctx->h_cfg[first + i];
         if (!out_host || !out_host[i]) continue;
-        const int pitch = c.outw * c.bpp;
-        void *map = (ctx->opt_host_rows && pitch > 0 && (pitch & 15) == 0 && (reinterpret_cast<uintptr_t>(c.out) & 15) == 0
+        const int row_bytes = c.outw * c.bpp;
+        void *map = (ctx->opt_host_rows && row_bytes > 0 && (c.out_pitch & 15) == 0 && (reinterpret_cast<uintptr_t>(c.out) & 15) == 0
                      && (long long) c.outh + (long long) c.v_fac >= kLines)
                         ? host_mapping(out_host[i]) : NULL;
         if (map && (reinterpret_cast<uintptr_t>(map) & 15) == 0) {
@@ -1095,7 +1140,11 @@ int crtx_frames_host(crtx_ctx *ctx, int first, int count, const crtx_source *src
             scatter += 1;
             continue;
         }
-        CUDA_TRY(cudaMemcpyAsync(out_host[i], c.out, (size_t) c.outw * c.outh * c.bpp, cudaMemcpyDeviceToHost, st));
+        if (c.out_pitch == row_bytes)
+            CUDA_TRY(cudaMemcpyAsync(out_host[i], c.out, (size_t) c.outw * c.outh * c.bpp, cudaMemcpyDeviceToHost, st));
+        else if (c.outh > 0) // the rows' bytes only: the padding between the host image's rows keeps its content
+            CUDA_TRY(cudaMemcpy2DAsync(out_host[i], (size_t) c.out_pitch, c.out, (size_t) c.out_pitch, (size_t) row_bytes, (size_t) c.outh,
+                                       cudaMemcpyDeviceToHost, st));
     }
     if (scatter) {
         CUDA_TRY(cudaMemcpyAsync(ctx->d_host_out + first, maps.data(), sizeof(unsigned char *) * count, cudaMemcpyHostToDevice, st));
@@ -1125,8 +1174,11 @@ int crtx_get_paths(crtx_ctx *ctx, int first, int count, int *paths, void *stream
         CUDA_TRY(cudaMemcpyAsync(tmp.data(), ctx->d_state + first, sizeof(MonState) * count, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
     }
-    for (int i = 0; i < count; i++)
-        paths[i] = (tmp[i].generic ? CRTX_PATH_GENERIC_EQ : 0) | (ctx->h_mod_staged[first + i] ? CRTX_PATH_STAGED_MOD : 0);
+    for (int i = 0; i < count; i++) {
+        const MonCfg &c = ctx->h_cfg[first + i];
+        paths[i] = (tmp[i].generic ? CRTX_PATH_GENERIC_EQ : 0) | (ctx->h_mod_staged[first + i] ? CRTX_PATH_STAGED_MOD : 0)
+                 | ((!kBloom && rows16_ok(c.out, c.out_pitch, c.outw, c.bpp)) ? CRTX_PATH_ROW16 : 0);
+    }
     return 0;
 }
 

@@ -60,6 +60,8 @@ struct crtx_ctx {
 };
 
 namespace crt {
+// bytes of one source row: w pixels of the format's size, 2-byte pixels on the NES (the dense pitch)
+inline long long src_row_bytes(int format, int w) { return (long long) w * (kIsNes ? 2 : bpp_of(format)); }
 int fail(const char *fmt, ...);
 void fill_src(SrcCfg *d, const crtx_source *s);
 int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cudaStream_t stream);
