@@ -47,6 +47,13 @@ __device__ __forceinline__ void pv1k_waves(int dci, int dcq, int hue, int satura
     }
 }
 
+// The rows the decoded lines spread over, as the reference computes them (crt_core.c:428-429): outh + v_fac in 32-bit
+// unsigned arithmetic (v_fac is unsigned), so a "negative" v_fac shrinks the span and may wrap it to anything.
+__host__ __device__ inline unsigned row_span(const MonCfg &c) { return (unsigned) c.outh + c.v_fac; }
+// Up to this span (k + 1) * span does not wrap for any line: beg and end never decrease from one line to the next.
+// Above it lines far apart can share rows, and the line passes take them one level at a time (k_sync, crtx.cu).
+constexpr unsigned kMonotonicSpan = 0xffffffffu / (unsigned) kLines;
+
 struct SyncLine { // what depends only on k, vsync and the detected field (not on the chains)
     short jl;   // signal line the decoded line reads: posmod(top + k + vsync, vres)
     short row;  // colour row: ypos % CC_VPER
@@ -59,7 +66,10 @@ struct SyncShared {
     int hs[kLines];     // hsync after each decoded line's search
     int ccr[kLines][kCc]; // burst-lock accumulator of the line's colour row after its 10 steps
     uint4 burst[kLines][kCc]; // the burst samples each decoded line locks onto, by carrier phase: bytes 0 .. 9 of [line][phase]
-    short rowlist[kVper > 3 ? kVper : 3][kLines]; // decoded lines of each colour row, in order
+    union {
+        short rowlist[kVper > 3 ? kVper : 3][kLines]; // decoded lines of each colour row, in order (step 3b)
+        short level[kLines]; // spans above kMonotonicSpan: the line pass each line runs in (filled after step 3b)
+    };
     int rowcount[kVper > 3 ? kVper : 3];
     int vs_found[2 * kVsyncWindow]; // per vsync candidate: crossing index or -1
     int generic;
@@ -591,6 +601,32 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
     __syncthreads();
     phase_mark(0, 8);
 
+    // Spans above kMonotonicSpan (a v_fac near 2^31, or one that wraps outh + v_fac to a huge span): beg and end wrap, so
+    // a line's rows may overlap those of any earlier line, not only of its neighbours.  The reference applies such lines
+    // in order.  Line k's level is 1 + the highest level of an earlier line whose written rows [beg, beg + nrows) overlap
+    // its own (0 if none does).  Lines of one level write disjoint rows, and the host runs one line pass per level, in
+    // order.  One warp walks the lines; it is a pathological geometry and this is not a fast path.
+    const bool by_level = row_span(cfg) > kMonotonicSpan;
+    if (by_level) {
+        if (warp == 0) {
+            for (int k = 0; k < kLines; k++) {
+                const SyncLine g = sh.ln[k];
+                if (g.beg < 0) continue;
+                const int e = g.beg + max(1, g.end - cfg.scanlines - g.beg); // crt_core.c:662-664
+                int lv = -1;
+                for (int j = lane; j < k; j += 32) {
+                    const SyncLine h = sh.ln[j];
+                    if (h.beg >= 0 && h.beg < e && g.beg < h.beg + max(1, h.end - cfg.scanlines - h.beg)) lv = max(lv, (int) sh.level[j]);
+                }
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) lv = max(lv, __shfl_xor_sync(0xffffffffu, lv, o));
+                if (lane == 0) sh.level[k] = (short) (lv + 1);
+                __syncwarp();
+            }
+        }
+        __syncthreads();
+    }
+
     // ---- 4. per-line records for k_lines (crt_core.c:452-454, 469-479), all threads
     int huesn, huecs;
     {
@@ -606,9 +642,10 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
         // When the output has fewer rows than there are decoded lines, consecutive lines land on the same
         // row and the reference applies them in order (each one blending onto, or overwriting, its
         // predecessor).  pad0 = position of this line within its run, pad1 = 1 for the run's last line;
-        // the host then launches the line kernel once per position (crtx.cu).
+        // the host then launches the line kernel once per position (crtx.cu).  Spans above kMonotonicSpan: pad0 = level.
         int rank = 0;
-        for (int j = k - 1; j >= 0 && g.beg >= 0 && sh.ln[j].beg == g.beg; j--) rank++;
+        if (by_level) rank = (g.beg >= 0) ? sh.level[k] : 0;
+        else for (int j = k - 1; j >= 0 && g.beg >= 0 && sh.ln[j].beg == g.beg; j--) rank++;
         rec.pad0 = rank;
         rec.pad1 = (k == kLines - 1 || sh.ln[k + 1].beg != g.beg) ? 1 : 0;
         rec.hsync = hs;

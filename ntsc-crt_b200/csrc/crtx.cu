@@ -472,16 +472,24 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
             // (flagged by k_sync); it is an empty pass otherwise
             // Fewer output rows than decoded lines: several lines share a row and must be applied in
             // order (crt_core.c:409-664 is a sequential loop).  Without blend only the last line of a run
-            // survives; with blend one launch per run position keeps the order.
-            const long long rows = (long long) c0.outh + (long long) c0.v_fac;
-            if (rows >= kLines) {
+            // survives; with blend one launch per run position keeps the order.  Spans above kMonotonicSpan: lines far
+            // apart share rows, one launch per level k_sync gave them (crt_sync.cuh), blend or not.
+            const unsigned rows = row_span(c0);
+            if (rows > kMonotonicSpan) {
+                for (int p = 0; p < kLines; p++) {
+                    geo.pass = p;
+                    launch_lines(ctx, hi - lo, lo, geo, stream);
+                    launched += 2;
+                }
+                launched -= 2;
+            } else if (rows >= (unsigned) kLines) {
                 geo.pass = -1;
                 launch_lines(ctx, hi - lo, lo, geo, stream);
             } else if (!geo.blend) {
                 geo.pass = -2;
                 launch_lines(ctx, hi - lo, lo, geo, stream);
             } else {
-                const int runs = (int) ((kLines + (rows > 0 ? rows : 1) - 1) / (rows > 0 ? rows : 1)) + 1;
+                const int runs = (int) ((kLines + (rows > 0 ? rows : 1u) - 1) / (rows > 0 ? rows : 1u)) + 1;
                 for (int p = 0; p < runs; p++) {
                     geo.pass = p;
                     launch_lines(ctx, hi - lo, lo, geo, stream);
@@ -1133,7 +1141,7 @@ int crtx_frames_host(crtx_ctx *ctx, int first, int count, const crtx_source *src
         if (!out_host || !out_host[i]) continue;
         const int row_bytes = c.outw * c.bpp;
         void *map = (ctx->opt_host_rows && row_bytes > 0 && (c.out_pitch & 15) == 0 && (reinterpret_cast<uintptr_t>(c.out) & 15) == 0
-                     && (long long) c.outh + (long long) c.v_fac >= kLines)
+                     && row_span(c) >= (unsigned) kLines && row_span(c) <= kMonotonicSpan) // every row written by one line
                         ? host_mapping(out_host[i]) : NULL;
         if (map && (reinterpret_cast<uintptr_t>(map) & 15) == 0) {
             maps[i] = static_cast<unsigned char *>(map);

@@ -67,10 +67,20 @@ def line_block(rank, world, lines):
     return shard_range(lines, rank, world)
 
 
+def row_span(outh, v_fac, lines):
+    """outh + v_fac as the reference computes it, in 32-bit unsigned arithmetic (v_fac is unsigned, crt_core.c:428):
+    a "negative" v_fac shrinks the span.  Raises ValueError for a span at which (k + 1) * span wraps 32 bits for some
+    line: lines far apart then share rows, and no partition into blocks of consecutive lines keeps their order."""
+    span = (outh + v_fac) & 0xFFFFFFFF
+    if span > 0xFFFFFFFF // lines:
+        raise ValueError("outh + v_fac = %d rows: the reference's row mapping wraps 32 bits, lines far apart share rows" % span)
+    return span
+
+
 def block_rows(lo, hi, outh, lines, v_fac=0):
     """Output rows [r0, r1) owned by the rank decoding lines [lo, hi): the rows its lines start on in an
     even field (crt_core.c:428), clipped to the image."""
-    span = outh + v_fac
+    span = row_span(outh, v_fac, lines)
     return min(outh, lo * span // lines), min(outh, hi * span // lines)
 
 
@@ -94,11 +104,12 @@ class ImageSharder:
         self.rank = rank if rank is not None else (dist.get_rank(group) if on else 0)
         self.image, self.lines, self.v_fac = image, lines, v_fac
         self.outh = image.shape[0]
-        if self.world > 1 and self.outh + v_fac < lines:
+        span = row_span(self.outh, v_fac, lines)
+        if self.world > 1 and span < lines:
             # several decoded lines share an output row and the reference applies them in line order
             # (crt_core.c:409-664 is a sequential loop): lines of two ranks would have to take turns on one row
             raise ValueError("scanline-block sharding needs at least one output row per decoded line: outh + v_fac = %d < %d lines"
-                             % (self.outh + v_fac, lines))
+                             % (span, lines))
         self.lo, self.hi = line_block(self.rank, self.world, lines)
         self.blocks = [block_rows(*line_block(r, self.world, lines), self.outh, lines, v_fac)
                        for r in range(self.world)]

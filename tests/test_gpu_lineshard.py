@@ -32,20 +32,20 @@ def test_blocks_of_the_newer_variants(variant, outw, outh, scanlines, blend, wor
     decode_one_image_in_blocks(variant, outw, outh, scanlines, blend, world)
 
 
-def decode_one_image_in_blocks(variant, outw, outh, scanlines, blend, world):
+def decode_one_image_in_blocks(variant, outw, outh, scanlines, blend, world, v_fac=0):
     import torch
     from ntsc_crt_b200 import capi
     img = S.rand_image(320, 240, seed=11)
     dimg = torch.from_numpy(img).cuda()
     ora = S.OracleEngine(variant, outw, outh)
-    ora.set(blend=blend, scanlines=scanlines)
+    ora.set(blend=blend, scanlines=scanlines, v_fac=v_fac)
     ranks = []
     for r in range(world):
         b = capi.Batch(variant, 1)
         out = torch.zeros(outh, outw, 4, dtype=torch.uint8, device="cuda")
-        b.set_monitor(0, out, fmt=layout.PIX_BGRA, noise=4, blend=blend, scanlines=scanlines)
+        b.set_monitor(0, out, fmt=layout.PIX_BGRA, noise=4, blend=blend, scanlines=scanlines, v_fac=v_fac)
         b.commit_monitors()
-        part = sharding.ImageSharder(out, b.spec.lines, rank=r, world=world)
+        part = sharding.ImageSharder(out, b.spec.lines, rank=r, world=world, v_fac=v_fac)
         part.apply(b)
         ranks.append((b, out, part))
     for it in range(6):

@@ -80,6 +80,26 @@ def test_line_blocks_and_row_ownership():
     assert sharding.block_rows(0, 30, 624, 240) == (0, 78)  # SURVEY 8e: 30 lines <-> 78 rows at 832x624
 
 
+def test_row_span_wraps_like_the_reference():
+    """outh + v_fac is 32-bit unsigned in the reference (crt_core.c:428): a "negative" v_fac shrinks the span, and a
+    span whose products wrap has no partition into blocks of consecutive lines"""
+    edge = (2**32 - 1) // 240
+    assert sharding.row_span(200, 2**32 - 60, 240) == 140
+    assert sharding.row_span(200, 100, 240) == 300
+    assert sharding.row_span(200, edge - 200, 240) == edge
+    assert sharding.block_rows(0, 120, 200, 240, v_fac=100) == (0, 150)
+    assert sharding.block_rows(120, 240, 200, 240, v_fac=100) == (150, 200)
+    for v_fac in (edge + 1 - 200, 2**31, 2**32 - 201):  # spans edge + 1, 2^31 + 200, 2^32 - 1
+        with pytest.raises(ValueError, match="wraps"):
+            sharding.block_rows(0, 120, 200, 240, v_fac=v_fac)
+        with pytest.raises(ValueError, match="wraps"):
+            sharding.ImageSharder(torch.zeros(200, 64, 4, dtype=torch.uint8), 240, rank=0, world=2, v_fac=v_fac)
+    with pytest.raises(ValueError, match="at least one output row"):  # shrunk below one row per line by the wrap
+        sharding.ImageSharder(torch.zeros(200, 64, 4, dtype=torch.uint8), 240, rank=0, world=2, v_fac=2**32 - 60)
+    part = sharding.ImageSharder(torch.zeros(200, 64, 4, dtype=torch.uint8), 240, rank=1, world=2, v_fac=100)
+    assert (part.r0, part.r1) == (150, 200)
+
+
 def _image_worker(rank, world, port, q, cfg):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank),
                       WORLD_SIZE=str(world), LOCAL_RANK=str(rank))

@@ -35,6 +35,7 @@ import test_gpu_still_cli as _still  # noqa: E402
 import test_gpu_video as _video  # noqa: E402
 import test_gpu_video_driver as _vdriver  # noqa: E402
 import test_gpu_video_convert_unmodified as _vconv  # noqa: E402
+import test_gpu_vfac as _vfac  # noqa: E402
 import test_gpu_wire as _wire  # noqa: E402
 
 
@@ -103,6 +104,7 @@ _adopt(_wire, "wire")
 _adopt(_bloom, "bloom")
 _adopt(_api, "api")
 _adopt(_guard, "guard")
+_adopt(_vfac, "vfac")
 test_cli_unmodified_cli_driver_is_byte_identical = _cli.test_unmodified_cli_driver_is_byte_identical
 _adopt(_still, "still")
 test_vconv_unmodified_video_convert_runs_against_the_library = _vconv.test_unmodified_video_convert_runs_against_the_library
@@ -169,7 +171,8 @@ def test_other_thread_schedules(schedule):
     GPU would expose as a race, fails here."""
     import subprocess
     env = dict(os.environ, SIMT_SCHEDULE=schedule)
-    sel = "bloom_batch or pv1k_batch or template_batch or wire_ppm or wire_fade or parity_batch_matches_independent_oracles or fullsize"
+    sel = ("bloom_batch or pv1k_batch or template_batch or wire_ppm or wire_fade or parity_batch_matches_independent_oracles or fullsize"
+           " or vfac_batch")
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-x", "-q", "-k", sel, "-p", "no:cacheprovider"],
                        env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, cwd=S.ROOT)
     assert r.returncode == 0, r.stdout[-3000:]
