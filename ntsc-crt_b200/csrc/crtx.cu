@@ -1038,9 +1038,10 @@ static int modulate_sources(crtx_ctx *ctx, int first, int count, const crtx_sour
         ctx->scratch_src[i].compact = (compact && compact[i]) ? 1 : 0;
     }
 #if (CRT_SYSTEM == CRT_SYSTEM_NTSCVHS)
-    { // the aberration draw happens on the device, from the monitor's rand() replica
+    { // the aberration draw happens on the device, from the monitor's rand() replica; a source of unknown format is not
+      // encoded and draws nothing (crt_ntscvhs.c:191-193 return before the draw at :205-207)
         std::vector<int> wants(count);
-        for (int i = 0; i < count; i++) wants[i] = src[i].do_aberration ? 1 : 0;
+        for (int i = 0; i < count; i++) wants[i] = (src[i].do_aberration && bpp_of(src[i].format) != 0) ? 1 : 0;
         CUDA_TRY(cudaMemcpyAsync(ctx->d_vhs_wants + first, wants.data(), sizeof(int) * count, cudaMemcpyHostToDevice,
                                  static_cast<cudaStream_t>(stream)));
         ctx->vhs_draw_aberration = 1;

@@ -36,6 +36,7 @@ import test_gpu_video as _video  # noqa: E402
 import test_gpu_video_driver as _vdriver  # noqa: E402
 import test_gpu_video_convert_unmodified as _vconv  # noqa: E402
 import test_gpu_vfac as _vfac  # noqa: E402
+import test_gpu_vhs as _vhs  # noqa: E402
 import test_gpu_wire as _wire  # noqa: E402
 
 
@@ -105,6 +106,7 @@ _adopt(_bloom, "bloom")
 _adopt(_api, "api")
 _adopt(_guard, "guard")
 _adopt(_vfac, "vfac")
+_adopt(_vhs, "vhs")
 test_cli_unmodified_cli_driver_is_byte_identical = _cli.test_unmodified_cli_driver_is_byte_identical
 _adopt(_still, "still")
 test_vconv_unmodified_video_convert_runs_against_the_library = _vconv.test_unmodified_video_convert_runs_against_the_library
@@ -116,6 +118,16 @@ def _bare(fn):
     g = types.FunctionType(fn.__code__, fn.__globals__, fn.__name__, fn.__defaults__, fn.__closure__)
     g.__doc__ = fn.__doc__
     return g
+
+
+@pytest.fixture(autouse=True)
+def small_vhs_runs(monkeypatch):
+    """tests/test_gpu_vhs.py with 4 monitors, 3 fields and one case of two calls per seed: every monitor and field costs
+    a whole interpreted noise pass here"""
+    monkeypatch.setattr(_vhs, "BATCH", 4)
+    monkeypatch.setattr(_vhs, "FIELDS", 3)
+    monkeypatch.setattr(_vhs, "SWEEP_CASES", 1)
+    monkeypatch.setattr(_vhs, "SWEEP_CALLS", 2)
 
 
 def test_fullsize_property_on_a_small_batch(monkeypatch):
@@ -172,7 +184,7 @@ def test_other_thread_schedules(schedule):
     import subprocess
     env = dict(os.environ, SIMT_SCHEDULE=schedule)
     sel = ("bloom_batch or pv1k_batch or template_batch or wire_ppm or wire_fade or parity_batch_matches_independent_oracles or fullsize"
-           " or vfac_batch")
+           " or vfac_batch or vhs_batch_many_generator_states")
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-x", "-q", "-k", sel, "-p", "no:cacheprovider"],
                        env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, cwd=S.ROOT)
     assert r.returncode == 0, r.stdout[-3000:]
