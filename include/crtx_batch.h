@@ -76,7 +76,12 @@ typedef struct crtx_line {
     int beg;        /* first output row, or -1 when the line is skipped (crt_core.c:431) */
     int end;        /* one past the last output row (crt_core.c:429,432) */
     int hsync;      /* after this line's search (crt_core.c:446) */
-    int pad0, pad1;
+    /* The order of lines that write the same rows.  With outh + v_fac (32-bit unsigned) below CRT_LINES, consecutive
+     * lines share rows: run_pos is this line's position among the lines that start on its row, and run_last is 1 for the
+     * last of them.  With outh + v_fac above 0xffffffff / CRT_LINES the rows wrap and lines far apart share rows:
+     * run_pos is then the line's wrap level, 1 + the highest level of an earlier line whose rows overlap its own.
+     * crtx_demodulate decodes the lines of one position (or level) per line pass, in order. */
+    int run_pos, run_last;
 } crtx_line;
 
 /* geometry of this library variant */

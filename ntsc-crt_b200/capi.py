@@ -66,7 +66,7 @@ class State(C.Structure):  # crtx_state
 
 class Line(C.Structure):  # crtx_line
     _fields_ = [("pos", C.c_int), ("wave0", C.c_int), ("wave1", C.c_int), ("beg", C.c_int),
-                ("end", C.c_int), ("hsync", C.c_int), ("pad0", C.c_int), ("pad1", C.c_int)]
+                ("end", C.c_int), ("hsync", C.c_int), ("run_pos", C.c_int), ("run_last", C.c_int)]
 
 
 CRT_EXPORTS = ("crt_init", "crt_resize", "crt_reset", "crt_modulate", "crt_demodulate",

@@ -81,9 +81,7 @@ __global__ void __launch_bounds__(kBloomWarps * 32) k_lines_bloom(const MonCfg *
     const int k = blockIdx.x * kBloomWarps + warp; // decoded line of this warp
     if (k >= kLines || geo.bpp == 0 || geo.outw <= 0) return;
     const LineRec rec = lines_base[(size_t) m * kLines + k];
-    const bool active = rec.beg >= 0 && k >= geo.line_lo && k < geo.line_hi
-                     && (geo.pass == -1 || (geo.pass == -2 ? rec.pad1 != 0 : rec.pad0 == geo.pass));
-    if (!active) return; // (warp-uniform)
+    if (!line_in_launch(k, rec, geo)) return; // (warp-uniform)
     const MonCfg cfg = cfgs[m];
     const BloomLine bl = bloom_base[(size_t) m * kLines + k];
     int *comp = reinterpret_cast<int *>(smem_raw) + warp * 3 * kBloomRow;
@@ -151,7 +149,7 @@ __global__ void __launch_bounds__(kBloomWarps * 32) k_lines_bloom(const MonCfg *
     fmt_positions(geo.out_format, rp, gp, bp);
     const int ap = (bpp == 4) ? (6 - rp - gp - bp) : -1; // the remaining byte of a 4-byte pixel
     unsigned char *row = cfg.out + (size_t) rec.beg * pitch;
-    const int nrows = max(1, rec.end - cfg.scanlines - rec.beg); // crt_core.c:662-664
+    const int nrows = rows_written(rec, cfg.scanlines);
     for (int j = lane; j < geo.outw; j += 32) {
         const unsigned pos = scan_l + (unsigned) j * (unsigned) bl.dx;
         const bool wr = f_lo >= 0 && pos < scan_r; // the written pixels are a prefix of the row (crt_core.c:555)

@@ -142,10 +142,33 @@ constexpr int kMaxOutw = 8192;
 struct LinesGeom { // uniform over a launch: host groups monitors by these (crtx.cu)
     int outw, out_format, bpp, blend;
     int pitch; // bytes between output rows (MonCfg::out_pitch, shared by every monitor of the launch)
-    int pass; // -1: every line; -2: only the last line of each shared-row run; >= 0: lines at this run position
+    int pass; // -1: every line; -2: only the last line of each shared-row run; >= 0: lines at this run position (level)
     int rnd; // 32768, passed as an argument so that it lives in a register (see pole())
     int dx;  // ((AV_LEN - 1) << 12) / outw (crt_core.c:527), computed by the host: no division in the kernels
     int line_lo, line_hi; // decoded lines [lo, hi) this launch may touch (scanline-block sharding across ranks)
+};
+
+// Whether a line pass decodes decoded line k, whose record is `l` (a LineRec, or anything with its beg, run_pos and
+// run_last): a line of the field (k < CRT_LINES) that the field shows (beg >= 0), inside the launch's window
+// [line_lo, line_hi), in the launch's pass.  (One flat condition: the kernels' code depends on its shape.)
+template <class Line> __device__ __forceinline__ bool line_in_launch(int k, const Line &l, const LinesGeom &geo)
+{
+    return k < kLines && l.beg >= 0 && k >= geo.line_lo && k < geo.line_hi
+        && (geo.pass == -1 || (geo.pass == -2 ? l.run_last != 0 : l.run_pos == geo.pass));
+}
+
+// A 4-byte CRT_PIX_FORMAT (crt_core.h:62-67): pack() puts 0x00RRGGBB in storage byte order with alpha byte `a` (0 or
+// 0xff); `alpha` is the alpha byte's mask and `blend_mask` keeps the halved colour bytes of a stored pixel, so the blend
+// is (old >> 1 & blend_mask) + new on whole words.
+template <int FMT> struct Fmt4 {
+    static constexpr unsigned sel_store = (FMT == CRT_PIX_FORMAT_RGBA) ? 0x4012u : (FMT == CRT_PIX_FORMAT_ARGB) ? 0x0124u
+                                        : (FMT == CRT_PIX_FORMAT_ABGR) ? 0x2104u : 0x4210u;
+    static constexpr unsigned alpha = (FMT == CRT_PIX_FORMAT_ARGB || FMT == CRT_PIX_FORMAT_ABGR) ? 0x000000ffu : 0xff000000u;
+    static constexpr unsigned blend_mask = 0x7f7f7f7fu & ~(alpha >> 1) & ~alpha;
+    static __device__ __forceinline__ unsigned pack(unsigned rgb, unsigned a = 0xffu)
+    {
+        return (FMT == CRT_PIX_FORMAT_BGRA) ? (a ? (rgb | alpha) : rgb) : __byte_perm(rgb, a, sel_store);
+    }
 };
 
 // The 16-byte row path of k_lines and k_lines_fir (and a condition of k_lines2): 4-byte pixels, rows of whole 16-byte
@@ -277,8 +300,7 @@ k_lines(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, co
     LineRec rec;
     rec.pos = 0; rec.wave0 = rec.wave1 = 0; rec.beg = -1; rec.end = -1; rec.hsync = 0;
     if (kline < kLines) rec = lines_base[(size_t) m * kLines + kline];
-    const bool active = (kline < kLines) && rec.beg >= 0 && kline >= geo.line_lo && kline < geo.line_hi
-                     && (geo.pass == -1 || (geo.pass == -2 ? rec.pad1 != 0 : rec.pad0 == geo.pass));
+    const bool active = line_in_launch(kline, rec, geo);
     const unsigned active_mask = __ballot_sync(0xffffffffu, active);
     if (active_mask == 0) return;
     const unsigned nactive = __popc(active_mask);
@@ -289,7 +311,7 @@ k_lines(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, co
     const int bright = cfg->brightness - (kBlack + cfg->black_point); // crt_core.c:304
     unsigned char *out = cfg->out;
     const int beg = active ? rec.beg : -1;
-    const int nrows = active ? max(1, rec.end - cfg->scanlines - rec.beg) : 0; // crt_core.c:662-664
+    const int nrows = active ? rows_written(rec, cfg->scanlines) : 0;
     const bool vec = (MODE != 2) && rows16_ok(out, geo.pitch, geo.outw, 4);
     LinesGeom fgeo = geo; // what the scalar flush branches on, pinned to the template mode
     fgeo.bpp = (MODE == 2) ? 3 : 4;
@@ -307,11 +329,8 @@ k_lines(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, co
         oldv[it] = make_uint4(0u, 0u, 0u, 0u);
     }
 
-    // storage byte order of 0x00RRGGBB (+ alpha 0xff) for the 4-byte formats (crt_core.h:62-67)
-    constexpr unsigned sel_store = (FMT == CRT_PIX_FORMAT_RGBA) ? 0x4012u : (FMT == CRT_PIX_FORMAT_ARGB) ? 0x0124u
-                                 : (FMT == CRT_PIX_FORMAT_ABGR) ? 0x2104u : 0x4210u;
-    constexpr unsigned alpha_ff = (FMT == CRT_PIX_FORMAT_ARGB || FMT == CRT_PIX_FORMAT_ABGR) ? 0x000000ffu : 0xff000000u;
-    constexpr unsigned blend_mask = (MODE != 2) ? (0x7f7f7f7fu & ~(alpha_ff >> 1) & ~alpha_ff) : 0x7f7f7fu;
+    using F = Fmt4<FMT>;
+    constexpr unsigned blend_mask = (MODE != 2) ? F::blend_mask : 0x7f7f7fu;
 
     const int dx = geo.dx; // crt_core.c:527
     // carrier value that multiplies sample i for I and for Q, by i % kCc
@@ -428,8 +447,8 @@ k_lines(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, co
                     px = yiq_pixel<kHalved>(ay, ai, aq, by, bi, bq, R, L, contrast);
                 }
                 if (MODE != 2) {
-                    px = (FMT == CRT_PIX_FORMAT_BGRA) ? (px | alpha_ff) : __byte_perm(px, 0xffu, sel_store);
-                    if (MODE == 1 && !kHalved) px = ((px >> 1) & blend_mask) | alpha_ff;
+                    px = F::pack(px);
+                    if (MODE == 1 && !kHalved) px = ((px >> 1) & blend_mask) | F::alpha;
                 } else if (geo.blend) {
                     px = (px >> 1) & 0x7f7f7fu;
                 }

@@ -147,8 +147,9 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
     const unsigned desc_a = smem_u32(desc);
 
     LineRec rec;
-    rec.pos = 0; rec.wave0 = rec.wave1 = 0; rec.beg = -1; rec.end = -1; rec.hsync = 0; rec.pad0 = rec.pad1 = 0;
+    rec.pos = 0; rec.wave0 = rec.wave1 = 0; rec.beg = -1; rec.end = -1; rec.hsync = 0; rec.run_pos = rec.run_last = 0;
     if (present) rec = lines_base[(size_t) m * kLines + kline];
+    // (the host launches this kernel only for pass -1, every line: the window alone, no pass test)
     const bool active = present && states[m].generic == 0 && rec.beg >= 0 && kline >= geo.line_lo && kline < geo.line_hi;
     const unsigned active_mask = __ballot_sync(0xffffffffu, active);
     if (active_mask == 0) return;
@@ -159,7 +160,7 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
     const int ybias = wmul(bright, 4 * 0xfff);                        // 4 * (L + R) * bright, see the header
     unsigned char *out = cfg->out;
     const int beg = active ? rec.beg : -1;
-    const int nrows = active ? max(1, rec.end - cfg->scanlines - rec.beg) : 0; // crt_core.c:662-664
+    const int nrows = active ? rows_written(rec, cfg->scanlines) : 0;
     const int pitch = geo.pitch;
     TileRows tr;
 #pragma unroll
@@ -172,11 +173,7 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
         tr.rows[it] = (lbeg >= 0) ? lrows : 0;
     }
 
-    // storage byte order of 0x00RRGGBB (+ alpha 0xff) for the 4-byte formats (crt_core.h:62-67)
-    constexpr unsigned sel_store = (FMT == CRT_PIX_FORMAT_RGBA) ? 0x4012u : (FMT == CRT_PIX_FORMAT_ARGB) ? 0x0124u
-                                 : (FMT == CRT_PIX_FORMAT_ABGR) ? 0x2104u : 0x4210u;
-    constexpr unsigned alpha_ff = (FMT == CRT_PIX_FORMAT_ARGB || FMT == CRT_PIX_FORMAT_ABGR) ? 0x000000ffu : 0xff000000u;
-    constexpr unsigned blend_mask = 0x7f7f7f7fu & ~(alpha_ff >> 1) & ~alpha_ff;
+    using F = Fmt4<FMT>;
     constexpr bool kHalved = MODE == 1; // when blending the channels are halved while they are clamped (yiq_to_rgb)
 
     // carrier value that multiplies sample i for I and for Q, by i % 4 (crt_core.c:538-543)
@@ -275,7 +272,7 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
                     const int y = wadd(wmul((int) ca.x, L4), wadd(wmul((int) cb.x, R4), ybias));                          \
                     unsigned px = yiq_to_rgb<kHalved>(y, wadd(wmul(ai, L4) >> 16, wmul(bi, R4) >> 16),                    \
                                                       wadd(wmul(aq, L4) >> 16, wmul(bq, R4) >> 16), contrast);            \
-                    px = (FMT == CRT_PIX_FORMAT_BGRA) ? (px | alpha_ff) : __byte_perm(px, 0xffu, sel_store);              \
+                    px = F::pack(px);                                                                                     \
                     sts_u1<J * 4>(tp_a, px);                                                                              \
                 }
                 CRT_L2_PIXEL(0) CRT_L2_PIXEL(1) CRT_L2_PIXEL(2) CRT_L2_PIXEL(3) CRT_L2_PIXEL(4) CRT_L2_PIXEL(5) CRT_L2_PIXEL(6) CRT_L2_PIXEL(7)
@@ -283,14 +280,14 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
                 blk++;
                 if (!(blk & 1)) { // two blocks = one 16-pixel tile
                     const int k0 = (blk - 2) * kL2Block;
-                    flush_tile<MODE == 1>(tile_q_a, old_a, tr, pitch, min(16, geo.outw - k0), min(16, geo.outw - k0 - 16), lane, blend_mask);
+                    flush_tile<MODE == 1>(tile_q_a, old_a, tr, pitch, min(16, geo.outw - k0), min(16, geo.outw - k0 - 16), lane, F::blend_mask);
                 }
             }
         }
     }
     if (blk & 1) { // odd number of blocks: the last tile holds one
         const int k0 = (blk - 1) * kL2Block;
-        flush_tile<MODE == 1>(tile_q_a, old_a, tr, pitch, geo.outw - k0, 0, lane, blend_mask);
+        flush_tile<MODE == 1>(tile_q_a, old_a, tr, pitch, geo.outw - k0, 0, lane, F::blend_mask);
     }
     cp_async_wait<0>();
     phase_mark(1, 14);

@@ -123,14 +123,11 @@ k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states
         if (kl < kLines) {
             const LineRec r = recs[kl];
             l.pos = r.pos; l.wave0 = r.wave0; l.wave1 = r.wave1; l.beg = r.beg; l.end = r.end;
-            l.run_pos = r.pad0; l.run_last = r.pad1;
+            l.run_pos = r.run_pos; l.run_last = r.run_last;
         }
         return l;
     };
-    auto is_active = [&](const FirLine &l) -> bool {
-        return l.index < kLines && l.beg >= 0 && l.index >= geo.line_lo && l.index < geo.line_hi
-            && (geo.pass == -1 || (geo.pass == -2 ? l.run_last != 0 : l.run_pos == geo.pass));
-    };
+    auto is_active = [&](const FirLine &l) -> bool { return line_in_launch(l.index, l, geo); };
 
     // everything the first line needs from global memory, requested together
     int kline = (int) blockIdx.x * kFirWarps + warp;
@@ -168,11 +165,8 @@ k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states
     const signed char *inp = inp_base + (size_t) m * kSignalBytes;
     const unsigned dx = (unsigned) (((kAvLen - 1) << 12) / geo.outw); // crt_core.c:527
     const int seg0 = min(geo.outw, kFirSeg);
-    constexpr unsigned sel_store = (FMT == CRT_PIX_FORMAT_RGBA) ? 0x4012u : (FMT == CRT_PIX_FORMAT_ARGB) ? 0x0124u
-                                 : (FMT == CRT_PIX_FORMAT_ABGR) ? 0x2104u : 0x4210u;
-    constexpr unsigned alpha_ff = (FMT == CRT_PIX_FORMAT_ARGB || FMT == CRT_PIX_FORMAT_ABGR) ? 0x000000ffu : 0xff000000u;
-    constexpr unsigned blend_mask = 0x7f7f7f7fu & ~(alpha_ff >> 1) & ~alpha_ff;
-    constexpr unsigned blend_even = 0xfefefefeu & ~alpha_ff; // (x & blend_even) >> 1 == (x >> 1) & blend_mask
+    using F = Fmt4<FMT>;
+    constexpr unsigned blend_even = 0xfefefefeu & ~F::alpha; // (x & blend_even) >> 1 == (x >> 1) & F::blend_mask
     int rp = 0, gp = 0, bp = 0;
     if (MODE == 2) fmt_positions(geo.out_format, rp, gp, bp);
 
@@ -220,7 +214,7 @@ k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states
         if (is_active(cur)) {
             unsigned char *sigbuf = stage + buf * kFirStage;
             const int a = cur.pos & 15;
-            const int nrows = max(1, cur.end - scanlines - cur.beg); // crt_core.c:662-664
+            const int nrows = rows_written(cur, scanlines);
             unsigned char *row0 = out + (size_t) cur.beg * pitch;
             mbar_wait(&bars[buf], (ph_sig >> buf) & 1);
             ph_sig ^= 1u << buf;
@@ -329,11 +323,11 @@ k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states
                     auto emit = [&](int u) {
                         const int j = u * 32 + lane;
                         const unsigned rgb = shade((unsigned) tab_slot[u], tab_r4[u]);
-                        unsigned v = (FMT == CRT_PIX_FORMAT_BGRA) ? rgb : __byte_perm(rgb, 0u, sel_store);
+                        unsigned v = F::pack(rgb, 0u);
                         if (MODE == 1) // crt_core.c:608 on whole words; the alpha byte is masked out and set
-                            v = alpha_ff + v + ((ob[j] & blend_even) >> 1);
+                            v = F::alpha + v + ((ob[j] & blend_even) >> 1);
                         else
-                            v |= alpha_ff;
+                            v |= F::alpha;
                         ob[j] = v;
                     };
 #pragma unroll
@@ -358,9 +352,9 @@ k_lines_fir(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states
                     unsigned rgb = pixel(px);
                     if (MODE != 2) {
                         unsigned char *p = row0 + (size_t) px * 4;
-                        unsigned v = (FMT == CRT_PIX_FORMAT_BGRA) ? (rgb | alpha_ff) : __byte_perm(rgb, 0xffu, sel_store);
+                        unsigned v = F::pack(rgb);
                         if (MODE == 1) // (rgb is already halved, v carries the alpha byte)
-                            v += (__ldcg(reinterpret_cast<const unsigned *>(p)) >> 1) & blend_mask;
+                            v += (__ldcg(reinterpret_cast<const unsigned *>(p)) >> 1) & F::blend_mask;
                         for (int r = 0; r < nrows; r++) __stcg(reinterpret_cast<unsigned *>(p + (size_t) r * pitch), v);
                     } else {
                         unsigned char *p = row0 + (size_t) px * 3;

@@ -53,6 +53,8 @@ __host__ __device__ inline unsigned row_span(const MonCfg &c) { return (unsigned
 // Up to this span (k + 1) * span does not wrap for any line: beg and end never decrease from one line to the next.
 // Above it lines far apart can share rows, and the line passes take them one level at a time (k_sync, crtx.cu).
 constexpr unsigned kMonotonicSpan = 0xffffffffu / (unsigned) kLines;
+// The rows a decoded line writes, from `beg` on (crt_core.c:662-664): `l` is anything with the line's beg and end.
+template <class Line> __device__ __forceinline__ int rows_written(const Line &l, int scanlines) { return max(1, l.end - scanlines - l.beg); }
 
 struct SyncLine { // what depends only on k, vsync and the detected field (not on the chains)
     short jl;   // signal line the decoded line reads: posmod(top + k + vsync, vres)
@@ -612,11 +614,11 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
             for (int k = 0; k < kLines; k++) {
                 const SyncLine g = sh.ln[k];
                 if (g.beg < 0) continue;
-                const int e = g.beg + max(1, g.end - cfg.scanlines - g.beg); // crt_core.c:662-664
+                const int e = g.beg + rows_written(g, cfg.scanlines);
                 int lv = -1;
                 for (int j = lane; j < k; j += 32) {
                     const SyncLine h = sh.ln[j];
-                    if (h.beg >= 0 && h.beg < e && g.beg < h.beg + max(1, h.end - cfg.scanlines - h.beg)) lv = max(lv, (int) sh.level[j]);
+                    if (h.beg >= 0 && h.beg < e && g.beg < h.beg + rows_written(h, cfg.scanlines)) lv = max(lv, (int) sh.level[j]);
                 }
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) lv = max(lv, __shfl_xor_sync(0xffffffffu, lv, o));
@@ -641,13 +643,14 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
         LineRec rec;
         // When the output has fewer rows than there are decoded lines, consecutive lines land on the same
         // row and the reference applies them in order (each one blending onto, or overwriting, its
-        // predecessor).  pad0 = position of this line within its run, pad1 = 1 for the run's last line;
-        // the host then launches the line kernel once per position (crtx.cu).  Spans above kMonotonicSpan: pad0 = level.
+        // predecessor).  run_pos = position of this line within its run, run_last = 1 for the run's last line;
+        // the host then launches the line kernel once per position (crtx.cu: line_passes).  Spans above kMonotonicSpan:
+        // run_pos = level.
         int rank = 0;
         if (by_level) rank = (g.beg >= 0) ? sh.level[k] : 0;
         else for (int j = k - 1; j >= 0 && g.beg >= 0 && sh.ln[j].beg == g.beg; j--) rank++;
-        rec.pad0 = rank;
-        rec.pad1 = (k == kLines - 1 || sh.ln[k + 1].beg != g.beg) ? 1 : 0;
+        rec.run_pos = rank;
+        rec.run_last = (k == kLines - 1 || sh.ln[k + 1].beg != g.beg) ? 1 : 0;
         rec.hsync = hs;
         rec.beg = g.beg;
         rec.end = g.end;

@@ -14,6 +14,7 @@
 #include <string.h>
 
 #include <cstddef>
+#include <type_traits>
 #include <vector>
 
 #include "crt_kernels.cuh"
@@ -73,36 +74,55 @@ static int upload_cfg(crtx_ctx *ctx, cudaStream_t stream)
     return 0;
 }
 
-template <bool FAST, int MODE, int FMT>
-static void launch_lines_one(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo, cudaStream_t stream)
+// ---- kernel instantiations.  A templated kernel takes its template arguments from runtime values (pixel format, blend,
+// colour): the with_* functions below call f with them as std::integral_constant.  A launch and crtx_create's
+// cudaFuncSetAttribute (set_smem_attrs) go through the same with_* function, so every instantiation a launch can pick
+// has its shared-memory size set, and no other instantiation exists.
+template <int V> using IntC = std::integral_constant<int, V>;
+
+// f(IntC<v>) for the runtime value v among Vs (nothing when it is none of them)
+template <int... Vs, class Fn> static void with_value(int v, Fn &&f) { (void) ((v == Vs && (f(IntC<Vs>()), true)) || ...); }
+
+// k_lines2, and k_lines / k_lines_fir on 4-byte pixels: f(IntC<MODE>, IntC<FMT>), MODE 0 without blend, 1 with blend
+template <class Fn> static void with_mode4(int format, int blend, Fn &&f)
 {
-    if constexpr (kConv) { // USE_CONVOLUTION build: one warp per decoded line (crt_lines_fir.cuh)
-        // about two waves of resident CTAs (2 per SM) over the whole launch, see k_lines_fir; the generic
-        // pass is normally empty and gets the smallest grid
-        int gx = FAST ? (4 * ctx->sm_count + count - 1) / count : 1;
-        gx = gx < 1 ? 1 : (gx > kFirGroups ? kFirGroups : gx);
-        const dim3 grid(gx, count);
-        k_lines_fir<FAST, MODE, FMT><<<grid, kFirWarps * 32, fir_smem<FAST>(), stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines,
-                                                                                      ctx->d_inp, lo, geo);
-    } else { // (only the kernel a build uses is instantiated)
-        k_lines<FAST, MODE, FMT><<<count, kLinesWarps * 32, lines_smem<FAST>(), stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines,
-                                                                                       ctx->d_inp, lo, geo);
-    }
+    with_value<CRT_PIX_FORMAT_ARGB, CRT_PIX_FORMAT_RGBA, CRT_PIX_FORMAT_ABGR, CRT_PIX_FORMAT_BGRA>(format, [&](auto fmt) {
+        with_value<0, 1>(blend ? 1 : 0, [&](auto mode) { f(mode, fmt); });
+    });
+}
+
+// k_lines / k_lines_fir: the 4-byte modes, and MODE 2 (FMT 0) for every other pixel size
+template <class Fn> static void with_mode(int bpp, int format, int blend, Fn &&f)
+{
+    if (bpp != 4) f(IntC<2>(), IntC<0>());
+    else with_mode4(format, blend, f);
+}
+
+// k_mod_picture_rgb_staged: f(IntC<FMT>, IntC<COLOR>) for a source's format and as_color
+template <class Fn> static void with_src_format(int format, int color, Fn &&f)
+{
+    with_value<0, 1, 2, 3, 4, 5>(format, [&](auto fmt) { with_value<0, 1>(color ? 1 : 0, [&](auto c) { f(fmt, c); }); });
 }
 
 template <bool FAST>
-static void launch_lines_mode(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo, cudaStream_t stream)
+static void launch_lines_k(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo, cudaStream_t stream)
 {
-    if (geo.bpp != 4) return launch_lines_one<FAST, 2, 0>(ctx, count, lo, geo, stream);
-#define LL(F)                                                                                     \
-    case F:                                                                                       \
-        if (geo.blend) launch_lines_one<FAST, 1, F>(ctx, count, lo, geo, stream);                 \
-        else launch_lines_one<FAST, 0, F>(ctx, count, lo, geo, stream);                           \
-        break;
-    switch (geo.out_format) {
-        LL(CRT_PIX_FORMAT_ARGB) LL(CRT_PIX_FORMAT_RGBA) LL(CRT_PIX_FORMAT_ABGR) LL(CRT_PIX_FORMAT_BGRA)
-    }
-#undef LL
+    with_mode(geo.bpp, geo.out_format, geo.blend, [&](auto mode, auto fmt) {
+        constexpr int M = decltype(mode)::value, F = decltype(fmt)::value;
+        if constexpr (kConv) { // USE_CONVOLUTION build: one warp per decoded line (crt_lines_fir.cuh)
+            // about two waves of resident CTAs (2 per SM) over the whole launch, see k_lines_fir; the generic
+            // pass is normally empty and gets the smallest grid
+            int gx = FAST ? (4 * ctx->sm_count + count - 1) / count : 1;
+            gx = gx < 1 ? 1 : (gx > kFirGroups ? kFirGroups : gx);
+            const dim3 grid(gx, count);
+            k_lines_fir<FAST, M, F><<<grid, kFirWarps * 32, fir_smem<FAST>(), stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines,
+                                                                                      ctx->d_inp, lo, geo);
+        } else { // (only the kernel a build uses is instantiated)
+            k_lines<FAST, M, F><<<count, kLinesWarps * 32, lines_smem<FAST>(), stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines,
+                                                                                       ctx->d_inp, lo, geo);
+        }
+        ctx->launches += 1;
+    });
 }
 
 // k_lines2 (crt_lines2.cuh): two monitors per CTA, tabulated resampler.  Taken when the whole run qualifies: the stock
@@ -118,42 +138,19 @@ static bool lines2_eligible(const crtx_ctx *ctx, int count, int lo, const LinesG
     return true;
 }
 
-template <int MODE, int FMT>
-static void launch_lines2_one(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo, cudaStream_t stream)
-{
-    k_lines2<MODE, FMT><<<(count + 1) / 2, kL2Threads, lines2_smem(geo.outw), stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines,
-                                                                                          ctx->d_inp, lo, count, geo);
-}
-
 static void launch_lines2(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo, cudaStream_t stream)
 {
-#define LL(F)                                                                  \
-    case F:                                                                    \
-        if (geo.blend) launch_lines2_one<1, F>(ctx, count, lo, geo, stream);   \
-        else launch_lines2_one<0, F>(ctx, count, lo, geo, stream);             \
-        break;
-    switch (geo.out_format) {
-        LL(CRT_PIX_FORMAT_ARGB) LL(CRT_PIX_FORMAT_RGBA) LL(CRT_PIX_FORMAT_ABGR) LL(CRT_PIX_FORMAT_BGRA)
-    }
-#undef LL
-}
-
-static cudaError_t lines2_attr_all()
-{
-    cudaError_t e = cudaSuccess;
-#define LA(M, T)                                                                                               \
-    if (e == cudaSuccess)                                                                                      \
-        e = cudaFuncSetAttribute(k_lines2<M, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, lines2_smem(kL2MaxOutw));
-#define LF(T) LA(0, T) LA(1, T)
-        LF(CRT_PIX_FORMAT_ARGB) LF(CRT_PIX_FORMAT_RGBA) LF(CRT_PIX_FORMAT_ABGR) LF(CRT_PIX_FORMAT_BGRA)
-#undef LF
-#undef LA
-    return e;
+    with_mode4(geo.out_format, geo.blend, [&](auto mode, auto fmt) {
+        constexpr int M = decltype(mode)::value, F = decltype(fmt)::value;
+        k_lines2<M, F><<<(count + 1) / 2, kL2Threads, lines2_smem(geo.outw), stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines,
+                                                                                         ctx->d_inp, lo, count, geo);
+        ctx->launches += 1;
+        ctx->lines2_launches += 1;
+    });
 }
 #else
 static bool lines2_eligible(const crtx_ctx *, int, int, const LinesGeom &) { return false; }
 static void launch_lines2(crtx_ctx *, int, int, const LinesGeom &, cudaStream_t) {}
-static cudaError_t lines2_attr_all() { return cudaSuccess; }
 #endif
 
 static void launch_lines(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo, cudaStream_t stream)
@@ -161,71 +158,63 @@ static void launch_lines(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo,
     if (kBloom) { // CRT_DO_BLOOM build: per-line resampling step, one kernel for every format (crt_bloom.cuh)
         k_lines_bloom<<<dim3(kBloomGroups, count), kBloomWarps * 32, kBloomSmem, stream>>>(
             ctx->d_cfg, ctx->d_lines, ctx->d_inp, static_cast<const BloomLine *>(ctx->d_bloom), lo, geo);
+        ctx->launches += 1;
         return;
     }
-    if (lines2_eligible(ctx, count, lo, geo)) {
-        launch_lines2(ctx, count, lo, geo, stream);
-        ctx->lines2_launches += 1;
-    } else {
-        launch_lines_mode<true>(ctx, count, lo, geo, stream);
-    }
-    launch_lines_mode<false>(ctx, count, lo, geo, stream); // the monitors k_sync flagged for the wrap-exact equaliser
-}
-
-template <bool FAST, int MODE, int FMT>
-static cudaError_t lines_attr()
-{
-    if constexpr (kConv)
-        return cudaFuncSetAttribute(k_lines_fir<FAST, MODE, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    fir_smem<FAST>());
-    else
-        return cudaFuncSetAttribute(k_lines<FAST, MODE, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    lines_smem<FAST>());
-}
-
-static cudaError_t lines_attr_all()
-{
-    cudaError_t e = cudaSuccess;
-#define LA(F, M, T)                                  \
-    if (e == cudaSuccess) e = lines_attr<F, M, T>();
-#define LF(T) LA(true, 0, T) LA(true, 1, T) LA(false, 0, T) LA(false, 1, T)
-    LF(CRT_PIX_FORMAT_ARGB) LF(CRT_PIX_FORMAT_RGBA) LF(CRT_PIX_FORMAT_ABGR) LF(CRT_PIX_FORMAT_BGRA)
-    LA(true, 2, 0) LA(false, 2, 0)
-#undef LF
-#undef LA
-    return e;
+    if (lines2_eligible(ctx, count, lo, geo)) launch_lines2(ctx, count, lo, geo, stream);
+    else launch_lines_k<true>(ctx, count, lo, geo, stream);
+    launch_lines_k<false>(ctx, count, lo, geo, stream); // the monitors k_sync flagged for the wrap-exact equaliser
 }
 
 #if CRT_B200_BANDLIMITED
-template <int FMT, bool COLOR>
-static void launch_mod_staged_one(crtx_ctx *ctx, int count, int first, cudaStream_t stream)
-{
-    k_mod_picture_rgb_staged<FMT, COLOR><<<count, 256, kModSSmem, stream>>>(ctx->d_src + first, ctx->d_cfg, ctx->d_analog, first);
-}
-
-// function attributes are per device: set by crtx_create for the context's device
-static cudaError_t mod_staged_attr_all()
-{
-    cudaError_t e = cudaSuccess;
-#define MA(F)                                                                                                                        \
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_mod_picture_rgb_staged<F, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kModSSmem);  \
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_mod_picture_rgb_staged<F, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kModSSmem);
-    MA(0) MA(1) MA(2) MA(3) MA(4) MA(5)
-#undef MA
-    return e;
-}
-
 static void launch_mod_staged(crtx_ctx *ctx, int format, bool color, int count, int first, cudaStream_t stream)
 {
-#define MS(F)                                                                        \
-    case F:                                                                          \
-        if (color) launch_mod_staged_one<F, true>(ctx, count, first, stream);        \
-        else launch_mod_staged_one<F, false>(ctx, count, first, stream);             \
-        break;
-    switch (format) { MS(0) MS(1) MS(2) MS(3) MS(4) MS(5) default: break; }
-#undef MS
+    with_src_format(format, color, [&](auto fmt, auto c) {
+        constexpr int F = decltype(fmt)::value;
+        constexpr bool COLOR = decltype(c)::value != 0;
+        k_mod_picture_rgb_staged<F, COLOR><<<count, 256, kModSSmem, stream>>>(ctx->d_src + first, ctx->d_cfg, ctx->d_analog, first);
+        ctx->launches += 1;
+    });
 }
 #endif
+
+// crtx_create: the dynamic shared memory of every instantiation the launches above can pick (function attributes are per
+// device), through the same with_* functions
+static cudaError_t set_smem_attrs()
+{
+    cudaError_t e = cudaSuccess;
+    auto set = [&](auto kernel, int smem) {
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    };
+    for (int format = CRT_PIX_FORMAT_RGB; format <= CRT_PIX_FORMAT_BGRA; format++) {
+        for (int flag = 0; flag < 2; flag++) { // blend, or the source's as_color
+            with_mode(bpp_of(format), format, flag, [&](auto mode, auto fmt) {
+                constexpr int M = decltype(mode)::value, F = decltype(fmt)::value;
+                if constexpr (kConv) {
+                    set(k_lines_fir<true, M, F>, fir_smem<true>());
+                    set(k_lines_fir<false, M, F>, fir_smem<false>());
+                } else {
+                    set(k_lines<true, M, F>, lines_smem<true>());
+                    set(k_lines<false, M, F>, lines_smem<false>());
+                }
+            });
+#if CRTX_HAS_LINES2
+            with_mode4(format, flag, [&](auto mode, auto fmt) {
+                constexpr int M = decltype(mode)::value, F = decltype(fmt)::value;
+                set(k_lines2<M, F>, lines2_smem(kL2MaxOutw));
+            });
+#endif
+#if CRT_B200_BANDLIMITED
+            with_src_format(format, flag, [&](auto fmt, auto c) {
+                constexpr int F = decltype(fmt)::value;
+                constexpr bool COLOR = decltype(c)::value != 0;
+                set(k_mod_picture_rgb_staged<F, COLOR>, kModSSmem);
+            });
+#endif
+        }
+    }
+    return e;
+}
 
 #if (CRT_SYSTEM == CRT_SYSTEM_NTSCVHS)
 // ---- glibc TYPE_3 rand() replica, host side (glibc 2.39 stdlib/random_r.c: srandom_r, random_r)
@@ -347,25 +336,25 @@ int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cuda
     {
         LaunchTimer lt(ctx, stream, 0);
         k_nes_table<<<count, 256, 0, stream>>>(ctx->d_src + first, ctx->d_cfg, ctx->d_state, ctx->d_nes_tab, first);
+        ctx->launches += 1;
         k_mod_nes<<<dim3(kNesParts, count), 256, 0, stream>>>(ctx->d_src + first, ctx->d_nes_tab, ctx->d_analog, first);
+        ctx->launches += 1;
     }
-    ctx->launches += 2;
 #elif (CRT_SYSTEM == CRT_SYSTEM_NESRGB)
     {
         LaunchTimer lt(ctx, stream, 0);
         k_mod_nesrgb<<<dim3(kNesRgbParts, count), 256, 0, stream>>>(ctx->d_src + first, ctx->d_cfg, ctx->d_state,
                                                                   ctx->d_analog, first);
+        ctx->launches += 1;
     }
-    ctx->launches += 1;
 #elif (CRT_SYSTEM == CRT_SYSTEM_SNES)
     {
         LaunchTimer lt(ctx, stream, 0);
         k_mod_snes<<<dim3(kSnesParts, count), 256, 0, stream>>>(ctx->d_src + first, ctx->d_cfg, ctx->d_state, ctx->d_analog,
                                                               first);
+        ctx->launches += 1;
     }
-    ctx->launches += 1;
 #else
-    int extra = 0;
     // (the staged kernel steps four samples per carrier period: not for the PV-1000's five, which takes the gather kernel)
     const bool staged = ctx->opt_mod_staged && (kCc == 4 || kCc == 5);
     // The gather kernel only runs for sources the staged one cannot take (their span does not fit a stage row), or for all of
@@ -379,7 +368,7 @@ int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cuda
     {
         LaunchTimer lt(ctx, stream, 0);
         k_mod_skeleton_rgb<<<count, 256, 0, stream>>>(ctx->d_src + first, ctx->d_state, ctx->d_analog, first);
-        extra += 1;
+        ctx->launches += 1;
     }
     {
         LaunchTimer lt(ctx, stream, 1);
@@ -387,23 +376,40 @@ int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cuda
             for (int lo = 0; lo < count;) {
                 int hi = lo + 1;
                 while (hi < count && src[hi].format == src[lo].format && (src[hi].as_color != 0) == (src[lo].as_color != 0)) hi++;
-                if (bpp_of(src[lo].format) != 0) {
-                    launch_mod_staged(ctx, src[lo].format, src[lo].as_color != 0, hi - lo, first + lo, stream);
-                    extra += 1;
-                }
+                if (bpp_of(src[lo].format) != 0) launch_mod_staged(ctx, src[lo].format, src[lo].as_color != 0, hi - lo, first + lo, stream);
                 lo = hi;
             }
         }
         if (gather) {
             k_mod_picture_rgb<<<count, 256, kModSmem, stream>>>(ctx->d_src + first, ctx->d_cfg, ctx->d_analog, first,
                                                                 staged ? 1 : 0);
-            extra += 1;
+            ctx->launches += 1;
         }
     }
-    ctx->launches += extra;
 #endif
     CUDA_TRY(cudaGetLastError());
     return 0;
+}
+
+// The line passes of a run of monitors that share this configuration, in order: LinesGeom::pass takes first, first + 1,
+// .. first + count - 1.  The reference applies the lines one after another (crt_core.c:409-664), so lines that write
+// the same rows go to different passes, in line order (k_sync numbers them: crtx_line::run_pos, run_last):
+//   rows >= CRT_LINES           every line owns its rows: one pass of every line (-1)
+//   fewer rows, no blend        only the last line of each run of lines on one row survives: one pass of those (-2)
+//   fewer rows, blend           one pass per position in the runs
+//   rows above kMonotonicSpan   lines far apart share rows: one pass per level, blend or not
+struct LinePasses {
+    int first, count;
+};
+
+static LinePasses line_passes(const MonCfg &c)
+{
+    const unsigned rows = row_span(c);
+    if (rows > kMonotonicSpan) return { 0, kLines };
+    if (rows >= (unsigned) kLines) return { -1, 1 };
+    if (!c.blend) return { -2, 1 };
+    const unsigned run = rows > 0 ? rows : 1u;
+    return { 0, (int) ((kLines + run - 1) / run) + 1 };
 }
 
 int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, const short *d_noise_terms)
@@ -416,6 +422,7 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
         dim3 tgrid((kInputSize + 255) / 256, count);
         LaunchTimer lt(ctx, stream, 2);
         k_noise_terms<<<tgrid, 256, 0, stream>>>(ctx->d_cfg, ctx->d_analog, ctx->d_inp, d_noise_terms, first);
+        ctx->launches += 1;
     } else { // batch path: the per-monitor rand() replica (crt_vhs.cuh)
         LaunchTimer lt(ctx, stream, 2);
         // two CTAs per monitor, side by side: (x, 0) the data-dependent tail of the field, (x, 1) its bulk
@@ -424,28 +431,28 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
                                                                        static_cast<const VhsJump *>(ctx->d_vhs_jump),
                                                                        ctx->d_vhs_raw + (size_t) first * kVhsTailRaw, ctx->d_analog,
                                                                        ctx->d_inp, first);
+        ctx->launches += 1;
         k_vhs_commit<<<(count * 32 + 255) / 256, 256, 0, stream>>>(static_cast<VhsRand *>(ctx->d_vhs_rand),
                                                                    static_cast<const VhsRand *>(ctx->d_vhs_rand_next), first, count);
+        ctx->launches += 1;
     }
-    int pre = 2;
 #else
-    (void) d_noise_terms;
-    int pre = 1; // the noise pass runs inside k_sync (crt_sync.cuh)
+    (void) d_noise_terms; // the noise pass runs inside k_sync (crt_sync.cuh)
 #endif
     {
         LaunchTimer lt(ctx, stream, 3);
         k_sync<<<count, kSyncThreads, kSyncSmem, stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines, ctx->d_analog, ctx->d_inp,
                                                            ctx->d_jump_lo, ctx->d_jump_hi, first, ctx->opt_generic);
+        ctx->launches += 1;
     }
     if (kBloom) { // line sums and the beam-energy chain: every line's resampling step and first sample
         LaunchTimer lt(ctx, stream, 3);
         k_bloom<<<count, 256, 0, stream>>>(ctx->d_cfg, ctx->d_lines, ctx->d_inp, static_cast<BloomLine *>(ctx->d_bloom), first);
-        pre += 1;
+        ctx->launches += 1;
     }
     // The line kernel takes the output geometry as launch-uniform arguments: split the range into
     // runs of monitors that share it (normally one run).  The row pitch is part of it: a batch of dense images, or of
     // tiles of one mosaic, has one pitch, so it costs no launch and the kernels read it from their parameters.
-    int launched = 0;
     for (int lo = first; lo < first + count;) {
         const MonCfg &c0 = ctx->h_cfg[lo];
         int hi = lo + 1;
@@ -466,42 +473,14 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
         geo.dx = c0.outw > 0 ? ((kAvLen - 1) << 12) / c0.outw : 0;
         geo.line_lo = ctx->opt_line_lo;
         geo.line_hi = ctx->opt_line_hi;
-        {
-            LaunchTimer lt(ctx, stream, 4);
-            // the second launch takes the monitors whose signal left the fast equaliser's exact range
-            // (flagged by k_sync); it is an empty pass otherwise
-            // Fewer output rows than decoded lines: several lines share a row and must be applied in
-            // order (crt_core.c:409-664 is a sequential loop).  Without blend only the last line of a run
-            // survives; with blend one launch per run position keeps the order.  Spans above kMonotonicSpan: lines far
-            // apart share rows, one launch per level k_sync gave them (crt_sync.cuh), blend or not.
-            const unsigned rows = row_span(c0);
-            if (rows > kMonotonicSpan) {
-                for (int p = 0; p < kLines; p++) {
-                    geo.pass = p;
-                    launch_lines(ctx, hi - lo, lo, geo, stream);
-                    launched += 2;
-                }
-                launched -= 2;
-            } else if (rows >= (unsigned) kLines) {
-                geo.pass = -1;
-                launch_lines(ctx, hi - lo, lo, geo, stream);
-            } else if (!geo.blend) {
-                geo.pass = -2;
-                launch_lines(ctx, hi - lo, lo, geo, stream);
-            } else {
-                const int runs = (int) ((kLines + (rows > 0 ? rows : 1u) - 1) / (rows > 0 ? rows : 1u)) + 1;
-                for (int p = 0; p < runs; p++) {
-                    geo.pass = p;
-                    launch_lines(ctx, hi - lo, lo, geo, stream);
-                    launched += 2;
-                }
-                launched -= 2;
-            }
+        LaunchTimer lt(ctx, stream, 4);
+        const LinePasses passes = line_passes(c0);
+        for (int p = 0; p < passes.count; p++) {
+            geo.pass = passes.first + p;
+            launch_lines(ctx, hi - lo, lo, geo, stream);
         }
-        launched += 2;
         lo = hi;
     }
-    ctx->launches += pre + launched;
     CUDA_TRY(cudaGetLastError());
     return 0;
 }
@@ -687,7 +666,7 @@ k_rows_scatter(const MonCfg *__restrict__ cfgs, const LineRec *__restrict__ line
     if (rec.beg < 0) return;
     const MonCfg cfg = cfgs[m];
     const int row_bytes = cfg.outw * cfg.bpp;
-    const int nrows = max(1, rec.end - cfg.scanlines - rec.beg); // crt_core.c:662-664
+    const int nrows = rows_written(rec, cfg.scanlines);
     for (int r = 0; r < nrows; r++) {
         const size_t off = (size_t) (rec.beg + r) * cfg.out_pitch;
         copy_row16(reinterpret_cast<const uint4 *>(cfg.out + off), reinterpret_cast<uint4 *>(host + off), row_bytes / 16, lane);
@@ -841,12 +820,10 @@ int crtx_create(crtx_ctx **out, int n)
         CTX_TRY(cudaFuncSetAttribute(k_noise_vhs, cudaFuncAttributeMaxDynamicSharedMemorySize, kVhsSmem));
     }
 #endif
-    CTX_TRY(lines_attr_all());
-    CTX_TRY(lines2_attr_all());
+    CTX_TRY(set_smem_attrs());
     CTX_TRY(cudaFuncSetAttribute(k_sync, cudaFuncAttributeMaxDynamicSharedMemorySize, kSyncSmem));
 #if CRT_B200_BANDLIMITED
     CTX_TRY(cudaFuncSetAttribute(k_mod_picture_rgb, cudaFuncAttributeMaxDynamicSharedMemorySize, kModSmem));
-    CTX_TRY(mod_staged_attr_all());
 #endif
 #undef CTX_TRY
     *out = ctx;

@@ -174,6 +174,78 @@ def test_the_interpreter_ran_kernels(simt_libs):
     assert lib.simt_launches() >= before + 4
 
 
+@pytest.mark.parametrize("variant", sorted(simt_build.variant_defines()))
+def test_launch_count_is_the_kernels_launched(simt_libs, variant, monkeypatch):
+    """crtx_launch_count counts every kernel a context launches: over modulates of mixed source formats, demodulates of
+    every kind of line-pass plan (a row per line and more, rows shared by consecutive lines with and without blend,
+    products that wrap) and crtx_frames_host, its delta equals the kernels the interpreter ran.  The drop-in calls
+    launch what a one-monitor context counts for the same field, except that on VHS the context also draws its noise
+    and aberration on the device (k_vhs_aberration, and k_noise_vhs + k_vhs_commit for the drop-in's k_noise_terms)."""
+    import ctypes as C
+    import torch
+    from ntsc_crt_b200 import layout
+    monkeypatch.setenv("SIMT_HOST_MAPPED", "1")  # crtx_frames_host takes its row copies
+    lib = C.CDLL(simt_libs(variant))
+    lib.simt_launches.restype = C.c_long
+    spec = layout.system_spec(variant)
+    nes = spec.system == layout.SYS_NES  # (NES sources are palette indices; NES-RGB ones are RGB images)
+    lines = spec.lines
+    edge = ((1 << 32) - 1) // lines
+
+    def counted(b, call):
+        ran, counts = lib.simt_launches(), b.launches
+        call()
+        return lib.simt_launches() - ran, b.launches - counts
+
+    outw, outh = 640, 200
+    # (format, span outh + v_fac, blend): one run of line passes each
+    monitors = [(layout.PIX_BGRA, lines, 1), (layout.PIX_RGB, 100, 1), (layout.PIX_ARGB, 100, 0), (layout.PIX_BGRA, edge + 1, 0)]
+    fmts = [layout.PIX_BGRA, layout.PIX_RGB, layout.PIX_RGBA, 9]  # (9: not a pixel format, encodes nothing)
+    b = capi.Batch(variant, len(monitors))
+    outs = [torch.zeros(outh, outw, layout.bpp4fmt(f), dtype=torch.uint8) for f, _, _ in monitors]
+    for i, (f, span, blend) in enumerate(monitors):
+        b.set_monitor(i, outs[i], fmt=f, noise=3, blend=blend, scanlines=1, v_fac=(span - outh) % (1 << 32))
+    b.commit_monitors()
+    for it in range(2):
+        for i in range(len(monitors)):
+            if nes:
+                img = torch.from_numpy(S.nes_image(seed=40 + i))
+                b.set_source(i, img, dot_crawl_offset=i % 3, reinit=int(it == 0))
+            else:
+                f = fmts[(i + it) % len(fmts)]
+                img = torch.from_numpy(S.rand_image(256, 224, bpp=layout.bpp4fmt(f) or 4, seed=40 + i))
+                b.set_source(i, img, format=f, as_color=(i + it) & 1, field=it & 1, frame=0, do_aberration=i & 1)
+        ran, counts = counted(b, b.modulate)
+        assert ran == counts and ran > 0, ("modulate", it, ran, counts)
+        ran, counts = counted(b, b.demodulate)
+        assert ran == counts and ran > 0, ("demodulate", it, ran, counts)
+    host = [torch.zeros(outh, outw, layout.bpp4fmt(f), dtype=torch.uint8) for f, _, _ in monitors]
+    ran, counts = counted(b, lambda: b.frames_host([h.data_ptr() for h in host]))
+    assert ran == counts and ran > 0, ("frames_host", ran, counts)
+    b.close()
+
+    # the drop-in interface against a one-monitor context, both after one field that uploads the configuration
+    img = S.nes_image(seed=50) if nes else S.rand_image(256, 224, seed=50)
+    kw = dict(dot_crawl_offset=1) if nes else dict(format=layout.PIX_BGRA, as_color=1, field=0, frame=0)
+    e = S.ProductEngine(variant, 320, 240)
+    e.set(blend=1, scanlines=1)
+    one = capi.Batch(variant, 1)
+    one.set_monitor(0, torch.zeros(240, 320, 4, dtype=torch.uint8), noise=3, blend=1, scanlines=1)
+    one.commit_monitors()
+    one.set_source(0, torch.from_numpy(img), **kw)
+    pair = []
+    for _ in range(2):
+        ran = lib.simt_launches()
+        e.modulate(img, **kw)
+        e.demodulate(3)
+        dropin = lib.simt_launches() - ran
+        ran, counts = counted(one, lambda: (one.modulate(), one.demodulate()))
+        assert ran == counts
+        pair.append((dropin, counts))
+    assert pair[1][0] + (2 if variant == "vhs" else 0) == pair[1][1], pair
+    one.close()
+
+
 @pytest.mark.skipif(os.environ.get("SIMT_SCHEDULE") is not None, reason="already running under an alternative schedule")
 @pytest.mark.parametrize("schedule", ["random:7"])
 def test_other_thread_schedules(schedule):
