@@ -77,36 +77,36 @@ __device__ __forceinline__ int warp_scan_incl(int v, int lane)
     return v;
 }
 
-// byte positions of R, G, B in a pixel of each CRT_PIX_FORMAT (crt_core.h:62-67)
-__device__ __forceinline__ void fmt_positions(int f, int &r, int &g, int &b)
-{
-    switch (f) {
-        case CRT_PIX_FORMAT_RGB:  r = 0; g = 1; b = 2; break;
-        case CRT_PIX_FORMAT_BGR:  r = 2; g = 1; b = 0; break;
-        case CRT_PIX_FORMAT_ARGB: r = 1; g = 2; b = 3; break;
-        case CRT_PIX_FORMAT_RGBA: r = 0; g = 1; b = 2; break;
-        case CRT_PIX_FORMAT_ABGR: r = 3; g = 2; b = 1; break;
-        default:                  r = 2; g = 1; b = 0; break; // BGRA
-    }
-}
-
 // =======================================================================================
-// encoder, RGB systems
+// encoder rules shared by the encoder kernels (and, for the picture size and source row, crtx_frames_host's row gather)
 // =======================================================================================
-#if CRT_B200_BANDLIMITED
 
 // Burst and carrier tables of the encoder, entry x of colour row `row`: sin() >> 10 of
 //   NTSC / VHS (crt_ntsc.c:174-188): burst hue + 90x + 33, I hue + 90x, Q hue + 90x - 90 (one row);
-//   template   (crt_template.c:166-183): with n = (row + dot_crawl_offset) * 180 + hue + 90x:
-//              burst n - 90 + HUE_OFFSET, I n, Q n + Q_OFFSET (rows 0 and 1);
+//   template   (crt_template.c:166-183), SNES (crt_snes.c:170-187): with n = (row + dot_crawl_offset) * 360 / VPER
+//              + hue + 90x: burst n - 90 + HUE_OFFSET, I n, Q n + Q_OFFSET (rows 0 and 1; SNES rows 0..2);
 //   PV-1000    (crt_pv1k.c:166-181): with n = (row + dot_crawl_offset) * 144 + hue + 72x (x < 5):
-//              burst n - 72, I n, Q n + 90 (rows 0..4).
+//              burst n - 72, I n, Q n + 90 (rows 0..4);
+//   NES-RGB    (crt_nesrgb.c:68-79): with n = (row + dot_crawl_offset) * 120 + 90x: burst hue + 90 + n + 33, I n,
+//              Q n - 90 (rows 0..2), colour or not;
+//   NES        (crt_nes.c:123-130): burst (hue + 90x + (row + dot_crawl_offset) * 120 + 33) % 360 (rows 0..2), no I / Q.
 __device__ __forceinline__ void enc_tables(const SrcCfg &s, int row, int x, int &burst, int &modI, int &modQ)
 {
     burst = modI = modQ = 0;
-    if (!s.as_color) return;
+    if (!kIsNes && !kIsNesRgb && !s.as_color) return;
     int sn, cs;
-    if (kIsPv1k) {
+    if (kIsNes) {
+        sincos14_d(sn, cs, (s.hue + x * 90 + (row + s.dot_crawl_offset) * 120 + 33) % 360 * 8192 / 180);
+        burst = sn >> 10;
+    } else if (kIsNesRgb) {
+        const int n = (row + s.dot_crawl_offset) * (360 / kVper) + x * (360 / 4);
+        sincos14_d(sn, cs, (s.hue + 90 + n + 33) * 8192 / 180);
+        burst = sn >> 10;
+        sincos14_d(sn, cs, n * 8192 / 180);
+        modI = sn >> 10;
+        sincos14_d(sn, cs, (n - 90) * 8192 / 180);
+        modQ = sn >> 10;
+    } else if (kIsPv1k) {
         const int step = 360 / 5;
         const int n = (row + s.dot_crawl_offset) * (360 * 2 / kVper) + s.hue + x * step;
         sincos14_d(sn, cs, (n - step) * 8192 / 180);
@@ -115,14 +115,14 @@ __device__ __forceinline__ void enc_tables(const SrcCfg &s, int row, int x, int 
         modI = sn >> 10;
         sincos14_d(sn, cs, (n + 90) * 8192 / 180);
         modQ = sn >> 10;
-    } else if (kIsTemp) {
+    } else if (kIsTemp || kIsSnes) {
         const int step = 360 / 4;
         const int n = (row + s.dot_crawl_offset) * (360 / kVper) + s.hue + x * step;
-        sincos14_d(sn, cs, (n - step + (-60)) * 8192 / 180); // HUE_OFFSET, crt_template.h:142
+        sincos14_d(sn, cs, (n - step + (kIsSnes ? 210 : -60)) * 8192 / 180); // HUE_OFFSET, crt_snes.h:99, crt_template.h:142
         burst = sn >> 10;
         sincos14_d(sn, cs, n * 8192 / 180);
         modI = sn >> 10;
-        sincos14_d(sn, cs, (n + (-90)) * 8192 / 180); // Q_OFFSET, crt_template.h:139
+        sincos14_d(sn, cs, (n + (-90)) * 8192 / 180); // Q_OFFSET, crt_snes.h:97, crt_template.h:139
         modQ = sn >> 10;
     } else {
         const int n = s.hue + x * 90;
@@ -134,6 +134,64 @@ __device__ __forceinline__ void enc_tables(const SrcCfg &s, int row, int x, int 
         modQ = sn >> 10;
     }
 }
+
+// the signal byte of burst table entry b (crt_ntsc.c:236-246); the burst lock is primed with 128 times it (crt_ntsc.c:325-329)
+__device__ __forceinline__ signed char burst_byte(int b) { return (signed char) ((kBlank + b * kBurst) >> 5); }
+
+// Picture size (crt_ntsc.c:131-133, 148-172; crt_snes.c:129-130, 144-168): kDestW x kDestH, or the image's own size where
+// that is smaller and the source asks for `raw`.  (Src: SrcCfg, or crtx_source on the host.)
+template <class Src> __host__ __device__ __forceinline__ void picture_size(const Src &s, int &destw, int &desth)
+{
+    destw = kDestW;
+    desth = kDestH;
+    if (s.raw) {
+        destw = min(s.w, kDestW);
+        desth = min(s.h, kDestH);
+    }
+}
+
+// Picture origin, centred in the active area (crt_ntsc.c:194-195), xo aligned to the carrier period: NTSC / VHS mask
+// (crt_ntsc.c:203), the template, PV-1000 and SNES subtract the remainder (crt_template.c:199, crt_pv1k.c:197,
+// crt_snes.c:201), which differs left of the line start.  (NES and NES-RGB do not centre, crt_nesrgb.c:86-90.)
+__device__ __forceinline__ void picture_origin(const SrcCfg &s, int destw, int desth, int &xo, int &yo)
+{
+    const int x = kAvBeg + s.xoffset + (kAvLen - destw) / 2;
+    xo = (kRowCarrier || kIsSnes) ? x - x % kCc : (x & ~3);
+    yo = kTop + s.yoffset + (kLines - desth) / 2;
+}
+
+// Source row of picture line y < desth of a band-limited system (crt_ntsc.c:258-266): y scaled to the image plus the
+// field's half-line offset.  The reference lets row == h read one row past the image (undefined); we clamp to the last
+// row instead.  A compact source holds exactly those rows, picture line y in row y (crtx_frames_host, k_rows_gather).
+__device__ __forceinline__ int source_row(int y, int h, int desth, int field, bool compact)
+{
+    int row = (int) (((long long) y * h) / desth) + (field * h + desth) / desth / 2;
+    if (row >= h) row = h - 1;
+    if (compact) row = y;
+    return row;
+}
+
+// phase inversion of the field (crt_ntsc.c:197-200); the template system and the PV-1000 walk colour rows instead
+__device__ __forceinline__ int phase_flip(const SrcCfg &s) { return kRowCarrier ? 0 : ((s.field & 1) == (s.frame & 1)); }
+
+// the rows of the RGB -> YIQ matrix (crt_ntsc.c:308-310), each sum >> 14
+constexpr int kYr = 19595, kYg = 38470, kYb = 7471;
+constexpr int kIr = 39059, kIg = -18022, kIb = -21103;
+constexpr int kQr = 13894, kQg = -34275, kQb = 20382;
+__device__ __forceinline__ void rgb_to_yiq(int r, int g, int b, int &fy, int &fi, int &fq)
+{
+    fy = (kYr * r + kYg * g + kYb * b) >> 14;
+    fi = (kIr * r + kIg * g + kIb * b) >> 14;
+    fq = (kQr * r + kQg * g + kQb * b) >> 14;
+}
+
+// the sample's level (crt_ntsc.c:316-321): black plus the signal scaled by white, clamped to 0..110 in one instruction
+__device__ __forceinline__ int ire_level(int sum, int white, int ire0) { return __vimin_s32_relu(ire0 + (wmul(sum, white) >> 10), 110); }
+
+// =======================================================================================
+// encoder, RGB systems
+// =======================================================================================
+#if CRT_B200_BANDLIMITED
 
 // first / last line of the equalising and vertical-sync groups (crt_ntsc.c:214,222; crt_template.h:149-156; the
 // PV-1000 has one equalising group and syncs at the bottom of the field, crt_pv1k.c:208,214)
@@ -147,8 +205,8 @@ __device__ __forceinline__ void mod_skeleton_lines(const SrcCfg &s, signed char 
                                                    int wstride, int lane)
 {
     static_assert(kHres % 2 == 0 && kAvBeg % 2 == 0, "pairs");
-    const int field = s.field & 1, frame = s.frame & 1;
-    const int flip = kRowCarrier ? 0 : (field == frame); // the template system and the PV-1000 have no phase inversion
+    const int field = s.field & 1;
+    const int flip = phase_flip(s);
     const int aberration = s.aberration;
     constexpr int H = kHres;
     for (int n = w0; n < kVres; n += wstride) {
@@ -172,7 +230,7 @@ __device__ __forceinline__ void mod_skeleton_lines(const SrcCfg &s, signed char 
             fill(kSyncBeg, kBwBeg, (n < kVres - aberration) ? kSync : kBlank); // crt_ntscvhs.c:234-238
             fill(kBwBeg, kCbBeg, kBlank);
             for (int t = kCbBeg + lane; t < kCbBeg + kBurstLen; t += 32) // crt_ntsc.c:236-246, crt_template.c:236-240
-                line[t] = (signed char) ((kBlank + burst[n % kVper][(t + flip * 2) % kCc] * kBurst) >> 5);
+                line[t] = burst_byte(burst[n % kVper][(t + flip * 2) % kCc]);
             fill(kCbBeg + kBurstLen, (n < kTop) ? H : kAvBeg, kBlank);
         }
     }
@@ -181,14 +239,11 @@ __device__ __forceinline__ void mod_skeleton_lines(const SrcCfg &s, signed char 
 // prime the burst lock (crt_ntsc.c:325-329 / crt_ntscvhs.c:332-336): thread e < CC_SAMPLES * CC_VPER writes ccf[e / CC][e % CC]
 __device__ __forceinline__ void mod_skeleton_prime(const SrcCfg &s, MonState *st, const int (*burst)[kCc], int e)
 {
-    const int field = s.field & 1, frame = s.frame & 1;
-    const int flip = kRowCarrier ? 0 : (field == frame);
     const int row = e / kCc, x = e % kCc;
     // template / PV-1000 (crt_template.c:239, 331-335; crt_pv1k.c:236, 326-330): every video line n stores its
     // burst bytes in row (n + 3) % VPER, so row r ends up with the bytes of the lines with n % VPER == r - 3
     const int from = kRowCarrier ? posmod(row - 3, kVper) : 0;
-    int p = (int) (signed char) ((kBlank + burst[from][(x + flip * 2) % kCc] * kBurst) >> 5);
-    st->ccf[row][x] = kIsVhs ? 0 : p * 128;
+    st->ccf[row][x] = kIsVhs ? 0 : burst_byte(burst[from][(x + phase_flip(s) * 2) % kCc]) * 128;
     if (kIsVhs && e == 0) st->hsync = 0; // crt_ntscvhs.c:258-259
 }
 
@@ -239,8 +294,51 @@ __device__ __forceinline__ void load_rgb(const unsigned char *data, size_t pix, 
     }
 }
 
-__host__ __device__ __forceinline__ bool mod_staged_ok(const SrcCfg &s, int destw);
-template <bool STAGED> __host__ __device__ __forceinline__ bool mod_takes(const SrcCfg &s);
+constexpr int kModSChunk = 32;                     // samples per chunk of the staged kernel (below)
+constexpr int kModSSpan = 192;                     // largest staged span the kernel accepts (incl. alignment slack)
+
+// Whether the staged picture kernel takes this source (the gather kernel takes the rest): the chunk's source span fits a
+// stage row, and the carrier has four or five samples per period.
+__host__ __device__ __forceinline__ bool mod_staged(const SrcCfg &s)
+{
+    int destw, desth;
+    picture_size(s, destw, desth);
+    const int bpp = bpp_of(s.format);
+    if (bpp == 0 || destw <= 0 || s.w <= 0 || (kCc != 4 && kCc != 5)) return false;
+    // widest source span of a chunk: ceil(32 * w / destw) + 1 pixels, plus 15 bytes of alignment
+    const long long span = ((long long) kModSChunk * s.w + destw - 1) / destw + 1;
+    // 4-byte pixels are read from the stage as words: every row must start on a 4-byte boundary
+    return span * bpp + 15 + 16 <= kModSSpan && s.w <= 65535
+        && (bpp != 4 || ((reinterpret_cast<uintptr_t>(s.data) | (uintptr_t) s.pitch) & 3) == 0);
+}
+
+// The picture kernels' carrier tables.  Five carrier phases (PV-1000): the phase of a sample is not a compile-time constant
+// of the 4-sample inner step, so threads 0 .. 24 put the tables of every colour row in shared memory, [I | Q][row][phase].
+__device__ __forceinline__ void carrier_smem(const SrcCfg &s, int (*mtab)[kVper][kCc])
+{
+    if (kCc == 5 && threadIdx.x < kCc * kVper) {
+        int b;
+        enc_tables(s, (int) threadIdx.x / kCc, (int) threadIdx.x % kCc, b, mtab[0][threadIdx.x / kCc][threadIdx.x % kCc],
+                   mtab[1][threadIdx.x / kCc][threadIdx.x % kCc]);
+    }
+}
+
+// Four phases: ph * ccmodI/Q (crt_ntsc.c:174-188, 197-200, 314-315) in registers; the template system takes the tables of
+// the lane's colour row `crow` (crt_template.c:266).  All 0 when `color` is false.
+__device__ __forceinline__ void carrier_lane(const SrcCfg &s, int crow, bool color, int (&mI)[4], int (&mQ)[4])
+{
+    const int ph = phase_flip(s) ? -1 : 1;
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        int b;
+        mI[k] = mQ[k] = 0;
+        if (color) {
+            enc_tables(s, crow, k, b, mI[k], mQ[k]);
+            mI[k] *= ph;
+            mQ[k] *= ph;
+        }
+    }
+}
 
 // (256, 2): its shared memory fits two CTAs per SM; a higher target spills the 64-bit row addresses
 __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb(const SrcCfg *__restrict__ srcs,
@@ -259,19 +357,11 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb(const SrcCfg *__rest
 
     const int bpp = bpp_of(s.format);
     if (bpp == 0) return;
-    if (skip_staged && mod_takes<true>(s)) return; // done by k_mod_picture_rgb_staged
-    int destw = kDestW, desth = kDestH;
-    if (s.raw) { // crt_ntsc.c:148-172
-        destw = min(s.w, kDestW);
-        desth = min(s.h, kDestH);
-    }
+    if (skip_staged && mod_staged(s)) return; // done by k_mod_picture_rgb_staged
+    int destw, desth, xo, yo;
+    picture_size(s, destw, desth);
     if (destw <= 0 || desth <= 0 || s.w <= 0 || s.h <= 0) return;
-    const int field = s.field & 1, frame = s.frame & 1;
-    const int flip = (field == frame);
-    const int ph = kRowCarrier ? 1 : (flip ? -1 : 1); // the template system and the PV-1000 walk colour rows instead (below)
-    const int xo_raw = kAvBeg + s.xoffset + (kAvLen - destw) / 2;
-    const int xo = kRowCarrier ? xo_raw - (xo_raw % kCc) : (xo_raw & ~3); // crt_template.c:199, crt_pv1k.c:197 / crt_ntsc.c:203
-    const int yo = kTop + s.yoffset + (kLines - desth) / 2;
+    picture_origin(s, destw, desth, xo, yo);
     const int white = kWhite * cfg.white_point / 100;
     const int ire0 = kBlack + cfg.black_point;
     int rp, gp, bp;
@@ -279,36 +369,19 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb(const SrcCfg *__rest
     const unsigned char *data = static_cast<const unsigned char *>(s.data);
     const bool aligned4 = (((reinterpret_cast<uintptr_t>(data) | (uintptr_t) s.pitch) & 3) == 0);
 
-    // five carrier phases (PV-1000): the phase of a sample is not a compile-time constant of the 4-sample inner
-    // step, so the tables live in shared memory, [I | Q][colour row][phase]
     __shared__ int mtab[2][kVper][kCc];
     if (kCc == 5) {
-        if (threadIdx.x < kCc * kVper) {
-            int b;
-            enc_tables(s, (int) threadIdx.x / kCc, (int) threadIdx.x % kCc, b, mtab[0][threadIdx.x / kCc][threadIdx.x % kCc],
-                       mtab[1][threadIdx.x / kCc][threadIdx.x % kCc]);
-        }
+        carrier_smem(s, mtab);
         __syncthreads(); // (every return above is block-uniform)
     }
     const int y = warp * 32 + lane; // this lane's picture line
     const int y0 = warp * 32;
     if (y0 >= desth) return;
-    // ph * ccmodI/Q (crt_ntsc.c:174-188, 314-315); template: the tables of this lane's colour row (crt_template.c:266)
     int mI[4], mQ[4];
     const int crow = kRowCarrier ? posmod(y + yo, kVper) : 0;
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        int b;
-        enc_tables(s, crow, k, b, mI[k], mQ[k]);
-        mI[k] *= ph;
-        mQ[k] *= ph;
-    }
+    carrier_lane(s, crow, true, mI, mQ);
     const int nlines = min(32, desth - y0);
-    // source row of this lane's line (crt_ntsc.c:258-266).  The reference lets row == h read one
-    // row past the image (undefined); we clamp to the last row instead.
-    int row = (int) (((long long) min(y, desth - 1) * s.h) / desth) + (field * s.h + desth) / desth / 2;
-    if (row >= s.h) row = s.h - 1;
-    if (s.compact) row = min(y, desth - 1); // crtx_frames_host staged exactly those rows, in line order (k_rows_gather)
+    const int row = source_row(min(y, desth - 1), s.h, desth, s.field & 1, s.compact);
 
     int hy = 0, hi = 0, hq = 0;
     for (int c0 = 0; c0 < destw; c0 += kModChunk) {
@@ -321,11 +394,9 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb(const SrcCfg *__rest
             const unsigned char *rowp = data + row_offset(__shfl_sync(0xffffffffu, row, l), s.pitch);
 #pragma unroll
             for (int half = 0; half < 2; half++) {
-                int r, g, b;
+                int r, g, b, fy, fi, fq;
                 load_rgb(rowp, half ? colb : cola, bpp, rp, gp, bp, aligned4, r, g, b);
-                int fy = (19595 * r + 38470 * g + 7471 * b) >> 14; // crt_ntsc.c:308-310
-                int fi = (39059 * r - 18022 * g - 21103 * b) >> 14;
-                int fq = (13894 * r - 34275 * g + 20382 * b) >> 14;
+                rgb_to_yiq(r, g, b, fy, fi, fq);
                 tile[l * kModTilePitch + lane + 32 * half] =
                     (unsigned) fy | (((unsigned) fi & 0x7ffu) << 10) | ((unsigned) fq << 21);
             }
@@ -347,9 +418,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb(const SrcCfg *__rest
                 const int p5 = (c0 + x4 + k) % kCc;
                 int ci = wmul(hi, kCc == 5 ? mtab[0][crow][p5] : mI[k]) >> 4;
                 int cq = wmul(hq, kCc == 5 ? mtab[1][crow][p5] : mQ[k]) >> 4;
-                int ire = ire0 + (wmul(hy + ci + cq, white) >> 10);
-                ire = __vimin_s32_relu(ire, 110); // clamp to 0..110 in one instruction
-                packed |= (unsigned) ire << (8 * k);
+                packed |= (unsigned) ire_level(hy + ci + cq, white, ire0) << (8 * k);
             }
             obuf[lane * kModOutPitch + (x4 >> 2)] = packed;
         }
@@ -386,8 +455,6 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb(const SrcCfg *__rest
 // (true of any cudaMalloc / torch allocation; include/crtx_batch.h).  A row's copy covers the 16-byte aligned superset
 // of its span, which may take in bytes of the padding between rows: they land in the stage and are never used.
 // ---------------------------------------------------------------------------------------
-constexpr int kModSChunk = 32;                     // samples per chunk
-constexpr int kModSSpan = 192;                     // largest staged span the kernel accepts (incl. alignment slack)
 // Stage bytes per line per chunk.  Every lane reads "its row, same column" at once, and rows start on
 // 16-byte boundaries, so the pitch decides the bank conflicts: 192 B (48 words) put all 32 lanes on 2
 // banks (16-way); 176 B (44 words) spreads them over 8 (4-way,
@@ -399,26 +466,6 @@ constexpr int kModSWarpSmem = 2 * 32 * kModSRow + 32 * kModSOutPitch * 4;
 // pixel from the first pixel of x's chunk, for whole chunks -- and each chunk's first and last source column.
 constexpr int kModSCols = (kDestW + kModSChunk - 1) / kModSChunk * kModSChunk;
 constexpr int kModSSmem = 8 * kModSWarpSmem + 8 * 2 * 8 + kModSCols * 4 + kModSCols / kModSChunk * 8;
-
-__host__ __device__ __forceinline__ bool mod_staged_ok(const SrcCfg &s, int destw)
-{
-    const int bpp = bpp_of(s.format);
-    if (bpp == 0 || destw <= 0 || s.w <= 0 || (kCc != 4 && kCc != 5)) return false; // (four or five samples per carrier period)
-    // widest source span of a chunk: ceil(32 * w / destw) + 1 pixels, plus 15 bytes of alignment
-    const long long span = ((long long) kModSChunk * s.w + destw - 1) / destw + 1;
-    // 4-byte pixels are read from the stage as words: every row must start on a 4-byte boundary
-    return span * bpp + 15 + 16 <= kModSSpan && s.w <= 65535
-        && (bpp != 4 || ((reinterpret_cast<uintptr_t>(s.data) | (uintptr_t) s.pitch) & 3) == 0);
-}
-
-template <bool STAGED>
-__host__ __device__ __forceinline__ bool mod_takes(const SrcCfg &s)
-{
-    int destw = kDestW;
-    if (s.raw) destw = s.w < kDestW ? s.w : kDestW;
-    return mod_staged_ok(s, destw) == STAGED;
-}
-
 
 // cr * R + cg * G + cb * B of a 4-byte pixel whose channels sit in bytes RP, GP, BP (crt_ntsc.c:308-310) as two-way dot
 // products on the pixel word itself (IDP.2A, crt_ptx.cuh): the coefficients of bytes (0, 1) and of bytes (2, 3) are packed as
@@ -477,7 +524,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const SrcCfg s = srcs[blockIdx.x];
-    if (!mod_takes<true>(s) || s.format != FMT || (s.as_color != 0) != COLOR) return;
+    if (!mod_staged(s) || s.format != FMT || (s.as_color != 0) != COLOR) return;
     const MonCfg cfg = cfgs[first + blockIdx.x];
     signed char *analog = analog_base + (size_t) (first + blockIdx.x) * kSignalBytes;
 
@@ -488,14 +535,9 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
     uint2 *spans = reinterpret_cast<uint2 *>(coltab + kModSCols);
 
     constexpr int bpp = (FMT <= 1) ? 3 : 4;
-    constexpr int rp = (FMT == 0 || FMT == 3) ? 0 : (FMT == 2) ? 1 : (FMT == 4) ? 3 : 2; // crt_core.h:62-67
-    constexpr int gp = (FMT == 2 || FMT == 4) ? 2 : 1;
-    constexpr int bp = (FMT == 0 || FMT == 3) ? 2 : (FMT == 2) ? 3 : (FMT == 4) ? 1 : 0;
-    int destw = kDestW, desth = kDestH;
-    if (s.raw) { // crt_ntsc.c:148-172
-        destw = min(s.w, kDestW);
-        desth = min(s.h, kDestH);
-    }
+    constexpr int rp = fmt_pos(FMT, 0), gp = fmt_pos(FMT, 1), bp = fmt_pos(FMT, 2);
+    int destw, desth;
+    picture_size(s, destw, desth);
     if (desth <= 0 || s.h <= 0) return;
     const int nchunks = (destw + kModSChunk - 1) / kModSChunk;
     // sample x reads source column (x * w) / destw (crt_ntsc.c:272), which depends on the monitor alone: tabulated once here
@@ -507,14 +549,8 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
         coltab[x] = (col - f0) * bpp;
         if ((x & (kModSChunk - 1)) == kModSChunk - 1) spans[x / kModSChunk] = make_uint2(f0, col);
     }
-    // five carrier phases (PV-1000): the phase of a sample is not a compile-time constant of the 4-sample inner step, so the
-    // tables live in shared memory, [I | Q][colour row][phase], as in the gather kernel
     __shared__ int mtab[2][kVper][kCc];
-    if (kCc == 5 && threadIdx.x < kCc * kVper) {
-        int b;
-        enc_tables(s, (int) threadIdx.x / kCc, (int) threadIdx.x % kCc, b, mtab[0][threadIdx.x / kCc][threadIdx.x % kCc],
-                   mtab[1][threadIdx.x / kCc][threadIdx.x % kCc]);
-    }
+    carrier_smem(s, mtab);
     __syncthreads(); // (every return above is block-uniform)
     const int y0 = warp * 32;
     if (y0 >= desth) return;
@@ -525,12 +561,8 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
         mbar_fence_init();
     }
     __syncwarp();
-    const int field = s.field & 1, frame = s.frame & 1;
-    const int flip = (field == frame);
-    const int ph = kRowCarrier ? 1 : (flip ? -1 : 1); // the template system and the PV-1000 walk colour rows instead (below)
-    const int xo_raw = kAvBeg + s.xoffset + (kAvLen - destw) / 2;
-    const int xo = kRowCarrier ? xo_raw - (xo_raw % kCc) : (xo_raw & ~3); // crt_template.c:199, crt_pv1k.c:197 / crt_ntsc.c:203
-    const int yo = kTop + s.yoffset + (kLines - desth) / 2;
+    int xo, yo;
+    picture_origin(s, destw, desth, xo, yo);
     const int white = kWhite * cfg.white_point / 100;
     const int ire0 = kBlack + cfg.black_point;
     const unsigned char *data = static_cast<const unsigned char *>(s.data);
@@ -538,25 +570,10 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
 
     const bool active = lane < nlines;
     const int y = y0 + min(lane, nlines - 1);
-    // ph * ccmodI/Q (crt_ntsc.c:174-188, 314-315); template: the tables of this lane's colour row (crt_template.c:266)
     int mI[4], mQ[4];
     const int crow = kRowCarrier ? posmod(y + yo, kVper) : 0;
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        int b;
-        mI[k] = mQ[k] = 0;
-        if (color) {
-            enc_tables(s, crow, k, b, mI[k], mQ[k]);
-            mI[k] *= ph;
-            mQ[k] *= ph;
-        }
-    }
-    // source row of this lane's line (crt_ntsc.c:258-266); row == h (one past the image, undefined in
-    // the reference) is clamped to the last row
-    int row = (int) (((long long) y * s.h) / desth) + (field * s.h + desth) / desth / 2;
-    if (row >= s.h) row = s.h - 1;
-    if (s.compact) row = y; // crtx_frames_host staged exactly those rows, in line order (k_rows_gather)
-    const unsigned char *rowp = data + row_offset(row, s.pitch);
+    carrier_lane(s, crow, color, mI, mQ);
+    const unsigned char *rowp = data + row_offset(source_row(y, s.h, desth, s.field & 1, s.compact), s.pitch);
 
     // chunk c covers samples [32c, 32c + 32); its span of source columns f0..f1 is staged from the 16-byte aligned address
     // at or below pixel f0.  Returns the offset of pixel f0 from that address.
@@ -577,10 +594,10 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
         return a;
     };
 
-    // the rows of the RGB -> YIQ matrix (crt_ntsc.c:308-310) for 4-byte pixels, see YiqDot
-    YiqDot<19595, 38470, 7471, rp, gp, bp> dot_y;
-    YiqDot<39059, -18022, -21103, rp, gp, bp> dot_i;
-    YiqDot<13894, -34275, 20382, rp, gp, bp> dot_q;
+    // the rows of the RGB -> YIQ matrix for 4-byte pixels, see YiqDot
+    YiqDot<kYr, kYg, kYb, rp, gp, bp> dot_y;
+    YiqDot<kIr, kIg, kIb, rp, gp, bp> dot_i;
+    YiqDot<kQr, kQg, kQb, rp, gp, bp> dot_q;
     if (bpp == 4) {
         const unsigned zero = (unsigned) first >> 31; // (0: the host keeps first in [0, 2^31))
         dot_y.init(zero);
@@ -653,7 +670,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
             }
 #pragma unroll
             for (int k = 0; k < 4; k++) {
-                int fy, fi = 0, fq = 0; // crt_ntsc.c:308-310
+                int fy, fi = 0, fq = 0;
                 if (bpp == 4) { // the matrix rows as dot products straight on the pixel word: no byte is ever extracted
                     fy = dot_y(pix[k]) >> 14;
                     if (color) {
@@ -661,12 +678,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
                         fq = dot_q(pix[k]) >> 14;
                     }
                 } else {
-                    const int r = rr[k], g = gg[k], b = bb[k];
-                    fy = (19595 * r + 38470 * g + 7471 * b) >> 14;
-                    if (color) {
-                        fi = (39059 * r - 18022 * g - 21103 * b) >> 14;
-                        fq = (13894 * r - 34275 * g + 20382 * b) >> 14;
-                    }
+                    rgb_to_yiq(rr[k], gg[k], bb[k], fy, fi, fq);
                 }
                 hy += wmul(fy - hy, kIirY) >> 11; // iirf, crt_ntsc.c:117-126
                 int sum = hy;
@@ -680,9 +692,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
                         sum += (wmul(hi, mI[k]) >> 4) + (wmul(hq, mQ[k]) >> 4);
                     }
                 }
-                int ire = ire0 + (wmul(sum, white) >> 10);
-                ire = __vimin_s32_relu(ire, 110); // clamp to 0..110 in one instruction
-                word |= (unsigned) ire << (8 * k);
+                word |= (unsigned) ire_level(sum, white, ire0) << (8 * k);
             }
             packed[g] = word;
         }
@@ -739,14 +749,13 @@ __global__ void __launch_bounds__(256) k_nes_table(const SrcCfg *__restrict__ sr
         ire += nes_square(p, phase) + nes_square(p, phase + 1) + nes_square(p, phase + 2) + nes_square(p, phase + 3);
         tab[e] = (signed char) ((wmul(ire, cfg.white_point) / 100) >> 12);
     }
-    if (tid < 12) { // burst rows (crt_nes.c:123-130) and the primed burst lock (crt_nes.c:196-200)
+    if (tid < 12) { // burst rows and the primed burst lock (crt_nes.c:196-200)
         const int row = tid >> 2, x = tid & 3;
-        int sn, cs;
-        const int deg = (s.hue + x * 90 + (row + s.dot_crawl_offset) * 120 + 33) % 360;
-        sincos14_d(sn, cs, deg * 8192 / 180);
-        const signed char v = (signed char) ((kBlank + (sn >> 10) * kBurst) >> 5);
+        int b, mi, mq;
+        enc_tables(s, row, x, b, mi, mq);
+        const signed char v = burst_byte(b);
         tab[512 * 12 + tid] = v;
-        states[first + m].ccf[row][x] = (int) v * 128;
+        states[first + m].ccf[row][x] = v * 128;
     }
 }
 
@@ -805,6 +814,44 @@ __global__ void __launch_bounds__(256) k_mod_nes(const SrcCfg *__restrict__ srcs
 
 #endif // NES
 
+#if (CRT_SYSTEM == CRT_SYSTEM_SNES) || (CRT_SYSTEM == CRT_SYSTEM_NESRGB)
+// Picture line of the RGB encoders without band-limit (SNES, NES-RGB): every sample is independent.  Sample x < destw of
+// `line` (from xo on) reads source pixel (x * w) / destw of `src_row` and takes the carrier of colour row `crow` at phase
+// (x + xo) % 4.  Thread tid takes samples tid, tid + 256, ... and issues all of its pixel fetches first.
+__device__ __forceinline__ void mod_line_unfiltered(const SrcCfg &s, const unsigned char *src_row, int destw, int xo,
+                                                    const int (*modI)[4], const int (*modQ)[4], int crow, int white,
+                                                    int ire0, signed char *line, int tid)
+{
+    const int bpp = bpp_of(s.format);
+    int rp, gp, bp;
+    fmt_positions(s.format, rp, gp, bp);
+    const bool word_pixels = (bpp == 4) && (((reinterpret_cast<uintptr_t>(s.data) | (uintptr_t) s.pitch) & 3) == 0);
+    constexpr int kPer = (kAvLen + 255) / 256; // samples per thread and line
+    unsigned px[kPer];
+#pragma unroll
+    for (int q = 0; q < kPer; q++) {
+        const int x = tid + q * 256;
+        px[q] = 0;
+        if (x < destw) {
+            const unsigned char *pix = src_row + (size_t) (((unsigned) x * (unsigned) s.w) / (unsigned) destw) * bpp;
+            if (word_pixels) px[q] = __ldg(reinterpret_cast<const unsigned *>(pix));
+            else px[q] = (unsigned) pix[0] | (unsigned) pix[1] << 8 | (unsigned) pix[2] << 16 | (bpp == 4 ? (unsigned) pix[3] << 24 : 0u);
+        }
+    }
+#pragma unroll
+    for (int q = 0; q < kPer; q++) {
+        const int x = tid + q * 256;
+        if (x >= destw) continue;
+        int fy, fi, fq;
+        rgb_to_yiq((px[q] >> (8 * rp)) & 0xff, (px[q] >> (8 * gp)) & 0xff, (px[q] >> (8 * bp)) & 0xff, fy, fi, fq);
+        const int xoff = (x + xo) % 4;
+        fi = wmul(fi, modI[crow][xoff]) >> 4;
+        fq = wmul(fq, modQ[crow][xoff]) >> 4;
+        line[x + xo] = (signed char) ire_level(fy + fi + fq, white, ire0);
+    }
+}
+#endif
+
 // =======================================================================================
 // encoder, SNES (crt_snes.c:125-327): the NTSC encoder's structure on the NES line layout, a burst and
 // carrier phase that walk a 3-line cycle (+ dot_crawl_offset), and NO band-limit (CRT_DO_BANDLIMITING 0,
@@ -826,42 +873,20 @@ __global__ void __launch_bounds__(256) k_mod_snes(const SrcCfg *__restrict__ src
     const MonCfg cfg = cfgs[first + m];
     signed char *analog = analog_base + (size_t) (first + m) * kSignalBytes;
 
-    if (tid < 12) { // crt_snes.c:170-187
+    if (tid < 12) {
         const int row = tid >> 2, x = tid & 3;
-        int bI = 0, bQ = 0, bB = 0;
-        if (s.as_color) {
-            const int step = 360 / 4;
-            const int n = (row + s.dot_crawl_offset) * (360 / kVper) + s.hue + x * step;
-            int sn, cs;
-            sincos14_d(sn, cs, (n - step + 210) * 8192 / 180); // HUE_OFFSET, crt_snes.h:99
-            bB = sn >> 10;
-            sincos14_d(sn, cs, n * 8192 / 180);
-            bI = sn >> 10;
-            sincos14_d(sn, cs, (n - 90) * 8192 / 180); // Q_OFFSET, crt_snes.h:97
-            bQ = sn >> 10;
-        }
-        modI[row][x] = bI;
-        modQ[row][x] = bQ;
-        burst[row][x] = bB;
+        enc_tables(s, row, x, burst[row][x], modI[row][x], modQ[row][x]);
         // crt_snes.c:246-248, 322-326: every video line re-primes the lock of its own row with its burst bytes
-        if (part == 0) states[first + m].ccf[row][x] = (int) (signed char) ((kBlank + bB * kBurst) >> 5) * 128;
+        if (part == 0) states[first + m].ccf[row][x] = burst_byte(burst[row][x]) * 128;
     }
     __syncthreads();
 
-    int destw = kDestW, desth = kDestH; // crt_snes.c:129-130, 144-168
-    if (s.raw) {
-        destw = min(s.w, kDestW);
-        desth = min(s.h, kDestH);
-    }
-    int xo = kAvBeg + s.xoffset + (kAvLen - destw) / 2;
-    const int yo = kTop + s.yoffset + (kLines - desth) / 2;
-    xo = xo - (xo % 4); // crt_snes.c:201
+    int destw, desth, xo, yo;
+    picture_size(s, destw, desth);
+    picture_origin(s, destw, desth, xo, yo);
     const int white = kWhite * cfg.white_point / 100;
     const int ire0 = kBlack + cfg.black_point;
-    int rp, gp, bp;
-    fmt_positions(s.format, rp, gp, bp);
     const unsigned char *data = static_cast<const unsigned char *>(s.data);
-    const bool word_pixels = (bpp == 4) && (((reinterpret_cast<uintptr_t>(data) | (uintptr_t) s.pitch) & 3) == 0);
 
     for (int n = part; n < kVres; n += kSnesParts) {
         signed char *line = analog + n * kHres;
@@ -878,7 +903,7 @@ __global__ void __launch_bounds__(256) k_mod_snes(const SrcCfg *__restrict__ src
             } else {
                 v = (t >= kSyncBeg && t < kBwBeg) ? kSync : kBlank;
                 write = (t < kAvBeg) || (n < kTop);
-                if (t >= kCbBeg && t < kCbBeg + kBurstLen) v = (kBlank + burst[n % kVper][t & 3] * kBurst) >> 5;
+                if (t >= kCbBeg && t < kCbBeg + kBurstLen) v = burst_byte(burst[n % kVper][t & 3]);
             }
             if (write) line[t] = (signed char) v;
         }
@@ -890,35 +915,7 @@ __global__ void __launch_bounds__(256) k_mod_snes(const SrcCfg *__restrict__ src
         if (xo < kAvBeg || n < kTop) __syncthreads(); // block-uniform condition
         int sy = (y * s.h) / desth;
         if (sy >= s.h) sy = s.h - 1; // (never taken for y < desth; the reference clamps to one row past the image)
-        const unsigned char *src_row = data + row_offset(sy, s.pitch);
-        const int ph = n % kVper;
-        constexpr int kPer = (kAvLen + 255) / 256; // samples per thread and line
-        unsigned px[kPer];
-#pragma unroll
-        for (int q = 0; q < kPer; q++) { // all of a thread's pixel fetches first
-            const int x = tid + q * 256;
-            px[q] = 0;
-            if (x < destw) {
-                const unsigned char *pix = src_row + (size_t) (((unsigned) x * (unsigned) s.w) / (unsigned) destw) * bpp;
-                if (word_pixels) px[q] = __ldg(reinterpret_cast<const unsigned *>(pix));
-                else px[q] = (unsigned) pix[0] | (unsigned) pix[1] << 8 | (unsigned) pix[2] << 16 | (bpp == 4 ? (unsigned) pix[3] << 24 : 0u);
-            }
-        }
-#pragma unroll
-        for (int q = 0; q < kPer; q++) {
-            const int x = tid + q * 256;
-            if (x >= destw) continue;
-            const int r = (px[q] >> (8 * rp)) & 0xff, g = (px[q] >> (8 * gp)) & 0xff, b = (px[q] >> (8 * bp)) & 0xff;
-            const int fy = (19595 * r + 38470 * g + 7471 * b) >> 14;
-            int fi = (39059 * r - 18022 * g - 21103 * b) >> 14;
-            int fq = (13894 * r - 34275 * g + 20382 * b) >> 14;
-            const int xoff = (x + xo) % 4;
-            fi = wmul(fi, modI[ph][xoff]) >> 4;
-            fq = wmul(fq, modQ[ph][xoff]) >> 4;
-            int ire = ire0 + (wmul(fy + fi + fq, white) >> 10);
-            ire = __vimin_s32_relu(ire, 110);
-            line[x + xo] = (signed char) ire;
-        }
+        mod_line_unfiltered(s, data + row_offset(sy, s.pitch), destw, xo, modI, modQ, n % kVper, white, ire0, line, tid);
     }
 }
 
@@ -944,28 +941,18 @@ __global__ void __launch_bounds__(256, 8) k_mod_nesrgb(const SrcCfg *__restrict_
     const MonCfg cfg = cfgs[first + m];
     signed char *analog = analog_base + (size_t) (first + m) * kSignalBytes;
 
-    if (tid < 12) { // crt_nesrgb.c:68-79
+    if (tid < 12) {
         const int row = tid >> 2, x = tid & 3;
-        const int n = (row + s.dot_crawl_offset) * (360 / kVper) + x * (360 / 4);
-        int sn, cs;
-        sincos14_d(sn, cs, (s.hue + 90 + n + 33) * 8192 / 180);
-        burst[row][x] = sn >> 10;
-        sincos14_d(sn, cs, n * 8192 / 180);
-        modI[row][x] = sn >> 10;
-        sincos14_d(sn, cs, (n - 90) * 8192 / 180);
-        modQ[row][x] = sn >> 10;
+        enc_tables(s, row, x, burst[row][x], modI[row][x], modQ[row][x]);
         // crt_nesrgb.c:106-110, 166-170: every picture line re-primes the lock of its row with its burst bytes
-        if (part == 0 && bpp != 0) states[first + m].ccf[row][x] = (int) (signed char) ((kBlank + burst[row][x] * kBurst) >> 5) * 128;
+        if (part == 0 && bpp != 0) states[first + m].ccf[row][x] = burst_byte(burst[row][x]) * 128;
     }
     __syncthreads();
 
     const int xo = (kAvBeg + s.xoffset) & ~3, yo = kTop + s.yoffset; // crt_nesrgb.c:86-90
     const int white = kWhite * cfg.white_point / 100;
     const int ire0 = kBlack + cfg.black_point;
-    int rp, gp, bp;
-    fmt_positions(s.format, rp, gp, bp);
     const unsigned char *data = static_cast<const unsigned char *>(s.data);
-    const bool word_pixels = (bpp == 4) && (((reinterpret_cast<uintptr_t>(data) | (uintptr_t) s.pitch) & 3) == 0);
 
     for (int n = part; n < kVres; n += kNesRgbParts) {
         signed char *line = analog + n * kHres;
@@ -978,39 +965,11 @@ __global__ void __launch_bounds__(256, 8) k_mod_nesrgb(const SrcCfg *__restrict_
         if (s.reinit) __syncthreads(); // (block-uniform) template before burst and picture
         if (tid < kBurstLen) { // crt_nesrgb.c:104-110
             const int t = kCbBeg + tid;
-            line[t] = (signed char) ((kBlank + burst[n % kVper][t & 3] * kBurst) >> 5);
+            line[t] = burst_byte(burst[n % kVper][t & 3]);
         }
         int sy = (y * s.h) / kLines;
         if (sy >= s.h) sy = s.h - 1; // (never taken; the reference clamps to one row past the image)
-        const unsigned char *src_row = data + row_offset(sy, s.pitch);
-        const int ph = n % kVper;
-        constexpr int kPer = (kAvLen + 255) / 256;
-        unsigned px[kPer];
-#pragma unroll
-        for (int q = 0; q < kPer; q++) { // all of a thread's pixel fetches first
-            const int x = tid + q * 256;
-            px[q] = 0;
-            if (x < kAvLen) {
-                const unsigned char *pix = src_row + (size_t) (((unsigned) x * (unsigned) s.w) / (unsigned) kAvLen) * bpp;
-                if (word_pixels) px[q] = __ldg(reinterpret_cast<const unsigned *>(pix));
-                else px[q] = (unsigned) pix[0] | (unsigned) pix[1] << 8 | (unsigned) pix[2] << 16 | (bpp == 4 ? (unsigned) pix[3] << 24 : 0u);
-            }
-        }
-#pragma unroll
-        for (int q = 0; q < kPer; q++) {
-            const int x = tid + q * 256;
-            if (x >= kAvLen) continue;
-            const int r = (px[q] >> (8 * rp)) & 0xff, g = (px[q] >> (8 * gp)) & 0xff, b = (px[q] >> (8 * bp)) & 0xff;
-            const int fy = (19595 * r + 38470 * g + 7471 * b) >> 14;
-            int fi = (39059 * r - 18022 * g - 21103 * b) >> 14;
-            int fq = (13894 * r - 34275 * g + 20382 * b) >> 14;
-            const int xoff = (x + xo) % 4;
-            fi = wmul(fi, modI[ph][xoff]) >> 4;
-            fq = wmul(fq, modQ[ph][xoff]) >> 4;
-            int ire = ire0 + (wmul(fy + fi + fq, white) >> 10);
-            ire = __vimin_s32_relu(ire, 110);
-            line[x + xo] = (signed char) ire;
-        }
+        mod_line_unfiltered(s, data + row_offset(sy, s.pitch), kAvLen, xo, modI, modQ, n % kVper, white, ire0, line, tid);
     }
 }
 

@@ -159,11 +159,12 @@ template <class Line> __device__ __forceinline__ bool line_in_launch(int k, cons
 
 // A 4-byte CRT_PIX_FORMAT (crt_core.h:62-67): pack() puts 0x00RRGGBB in storage byte order with alpha byte `a` (0 or
 // 0xff); `alpha` is the alpha byte's mask and `blend_mask` keeps the halved colour bytes of a stored pixel, so the blend
-// is (old >> 1 & blend_mask) + new on whole words.
+// is (old >> 1 & blend_mask) + new on whole words.  sel_store puts rgb's byte 2 (R), 1 (G), 0 (B) and `a` (selector 4)
+// at the format's byte positions (fmt_pos).
 template <int FMT> struct Fmt4 {
-    static constexpr unsigned sel_store = (FMT == CRT_PIX_FORMAT_RGBA) ? 0x4012u : (FMT == CRT_PIX_FORMAT_ARGB) ? 0x0124u
-                                        : (FMT == CRT_PIX_FORMAT_ABGR) ? 0x2104u : 0x4210u;
-    static constexpr unsigned alpha = (FMT == CRT_PIX_FORMAT_ARGB || FMT == CRT_PIX_FORMAT_ABGR) ? 0x000000ffu : 0xff000000u;
+    static constexpr unsigned sel_store = (2u << (4 * fmt_pos(FMT, 0))) | (1u << (4 * fmt_pos(FMT, 1)))
+                                        | (0u << (4 * fmt_pos(FMT, 2))) | (4u << (4 * fmt_pos(FMT, 3)));
+    static constexpr unsigned alpha = 0xffu << (8 * fmt_pos(FMT, 3));
     static constexpr unsigned blend_mask = 0x7f7f7f7fu & ~(alpha >> 1) & ~alpha;
     static __device__ __forceinline__ unsigned pack(unsigned rgb, unsigned a = 0xffu)
     {

@@ -228,7 +228,27 @@ constexpr Affine kLcgField = lcg_jump((uint32_t) kInputSize); // one whole crt_d
 static_assert(kLcgField.mul == 0x5535b491u && kLcgField.add == 0xf58bfa78u, "SURVEY.md 7.2 K1");
 #endif
 
-// pixel formats (crt_core.h:62-67): byte positions of R, G, B, A(-1 = none)
+// pixel formats (crt_core.h:62-67): bytes per pixel, and the byte positions of R, G, B in a pixel (a 4-byte format's
+// alpha takes the remaining byte, 6 - r - g - b)
 __host__ __device__ inline int bpp_of(int f) { return (f == 0 || f == 1) ? 3 : ((f >= 2 && f <= 5) ? 4 : 0); }
+constexpr __host__ __device__ void fmt_positions(int f, int &r, int &g, int &b)
+{
+    switch (f) {
+        case CRT_PIX_FORMAT_RGB:  r = 0; g = 1; b = 2; break;
+        case CRT_PIX_FORMAT_BGR:  r = 2; g = 1; b = 0; break;
+        case CRT_PIX_FORMAT_ARGB: r = 1; g = 2; b = 3; break;
+        case CRT_PIX_FORMAT_RGBA: r = 0; g = 1; b = 2; break;
+        case CRT_PIX_FORMAT_ABGR: r = 3; g = 2; b = 1; break;
+        default:                  r = 2; g = 1; b = 0; break; // BGRA
+    }
+}
+// the byte position of channel c (0 R, 1 G, 2 B, 3 alpha) at compile time
+constexpr int fmt_pos(int f, int c)
+{
+    int p[4] = { 0, 0, 0, 0 };
+    fmt_positions(f, p[0], p[1], p[2]);
+    p[3] = 6 - p[0] - p[1] - p[2];
+    return p[c];
+}
 
 } // namespace crt

@@ -358,10 +358,10 @@ int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cuda
     // (the staged kernel steps four samples per carrier period: not for the PV-1000's five, which takes the gather kernel)
     const bool staged = ctx->opt_mod_staged && (kCc == 4 || kCc == 5);
     // The gather kernel only runs for sources the staged one cannot take (their span does not fit a stage row), or for all of
-    // them when staging is off: the host can tell (mod_takes is a pure function of the settings), so the usual call saves a launch.
+    // them when staging is off: the host can tell (mod_staged is a pure function of the settings), so the usual call saves a launch.
     bool gather = !staged;
     for (int i = 0; i < count; i++) {
-        const bool takes = bpp_of(src[i].format) != 0 && staged && mod_takes<true>(src[i]);
+        const bool takes = bpp_of(src[i].format) != 0 && staged && mod_staged(src[i]);
         if (bpp_of(src[i].format) != 0 && staged && !takes) gather = true;
         ctx->h_mod_staged[first + i] = takes ? 1 : 0;
     }
@@ -647,8 +647,7 @@ __global__ void __launch_bounds__(kRowWarps * 32) k_rows_gather(const RowGather 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int y = blockIdx.x * kRowWarps + warp;
     if (!j.src || y >= j.desth) return;
-    int row = (int) (((long long) y * j.h) / j.desth) + (j.field * j.h + j.desth) / j.desth / 2; // crt_ntsc.c:258-266
-    if (row >= j.h) row = j.h - 1; // (as the encoder kernels: the reference's one-row over-read is not reproduced)
+    const int row = source_row(y, j.h, j.desth, j.field, false); // the rows the encoder kernels read
     copy_row16(reinterpret_cast<const uint4 *>(j.src + (size_t) row * j.src_pitch),
                reinterpret_cast<uint4 *>(j.dst + (size_t) y * j.row_bytes), j.row_bytes / 16, lane);
 }
@@ -1090,7 +1089,8 @@ int crtx_frames_host(crtx_ctx *ctx, int first, int count, const crtx_source *src
             j.src_pitch = pitch;
             dev[i].pitch = j.row_bytes;
             j.h = src[i].h;
-            j.desth = src[i].raw ? (src[i].h < kDestH ? src[i].h : kDestH) : kDestH; // crt_ntsc.c:132-133, 163-172
+            int destw;
+            picture_size(src[i], destw, j.desth);
             j.field = src[i].field & 1;
             compact[i] = 1;
             row_jobs += 1;

@@ -335,7 +335,7 @@ def dest_width(variant):
 
 
 def staged_ok(w, destw, bpp):
-    """mod_staged_ok (crt_kernels.cuh): the widest source span of a chunk, ceil(32 w / destw) + 1 pixels, plus 15 bytes of
+    """mod_staged (crt_kernels.cuh): the widest source span of a chunk, ceil(32 w / destw) + 1 pixels, plus 15 bytes of
     alignment slack and 16 of copy rounding, fits the 192-byte limit"""
     span = (CHUNK * w + destw - 1) // destw + 1
     return span * bpp + 15 + 16 <= K_SPAN
