@@ -18,6 +18,8 @@
  *      CRT_SYSTEM 1 (CRT_CHROMA_PATTERN 2)   libcrt_b200_nes.so
  *      CRT_SYSTEM 1, CRT_CHROMA_PATTERN 0    libcrt_b200_nes_p0.so
  *      CRT_SYSTEM 1, CRT_CHROMA_PATTERN 1    libcrt_b200_nes_p1.so
+ *      CRT_SYSTEM 1, NES_BORDER 1            libcrt_b200_nes_border.so (chroma pattern 2)
+ *      CRT_SYSTEM 1, CRT_CHROMA_PATTERN 0, NES_BORDER 1  libcrt_b200_nes_p0_border.so
  *      CRT_SYSTEM 3                          libcrt_b200_snes.so
  *      CRT_SYSTEM 6 (CRT_CHROMA_PATTERN 2)   libcrt_b200_nesrgb.so
  *      CRT_SYSTEM 6, CRT_CHROMA_PATTERN 0 / 1  libcrt_b200_nesrgb_p0.so / libcrt_b200_nesrgb_p1.so
@@ -329,6 +331,16 @@ struct NTSC_SETTINGS {
 
 #else
 #error "crt_b200: unknown CRT_SYSTEM (0 NTSC, 1 NES, 2 PV1K, 3 SNES, 4 TEMP, 5 NTSCVHS, 6 NESRGB)"
+#endif
+
+/* crt_nes.c:64-69 (an unguarded #define there, off): the NES encoder draws lines CRT_TOP .. CRT_BOT + 2 from LAV_BEG
+ * on in settings.border_color before the picture.  The libraries built with NES_BORDER 1 (libcrt_b200_nes_border.so,
+ * libcrt_b200_nes_p0_border.so) do; every other NES build ignores border_color, as the reference does. */
+#ifndef NES_BORDER
+#define NES_BORDER 0
+#endif
+#if NES_BORDER && (CRT_SYSTEM != CRT_SYSTEM_NES)
+#error "NES_BORDER is a switch of the NES encoder (crt_nes.c:64-69)"
 #endif
 
 #define CRT_INPUT_SIZE (CRT_HRES * CRT_VRES)

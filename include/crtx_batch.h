@@ -49,6 +49,7 @@ typedef struct crtx_source {
     int dot_crawl_offset; /* CRT_SYSTEM_NES, _NESRGB, _SNES, _TEMP, _PV1K */
     int reinit;           /* CRT_SYSTEM_NES: settings.field_initialized was 0 */
     int pitch;            /* bytes between the starts of two source rows; 0 = dense (w * bpp, NES w * 2) */
+    unsigned border_color; /* CRT_SYSTEM_NES built with NES_BORDER 1 (crtx_nes_border()) only: a 9-bit PPU pixel */
 } crtx_source;
 
 /* Row pitches.  A pitch of 0 means dense rows, which is what a zeroed struct gives.  Otherwise the pitch must be at
@@ -87,6 +88,7 @@ typedef struct crtx_line {
 /* geometry of this library variant */
 int crtx_system(void);          /* CRT_SYSTEM */
 int crtx_chroma_pattern(void);  /* CRT_CHROMA_PATTERN */
+int crtx_nes_border(void);      /* NES_BORDER: 1 if the NES encoder draws the border colour (crt_nes.c:64-69) */
 int crtx_hres(void);            /* CRT_HRES */
 int crtx_input_size(void);      /* CRT_INPUT_SIZE */
 int crtx_lines(void);           /* CRT_LINES */

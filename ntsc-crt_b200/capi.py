@@ -15,6 +15,11 @@ from . import LIB_DIR
 from . import layout
 
 VARIANTS = ("ntsc", "ntsc_conv", "ntsc_conv6", "ntsc_conv5", "ntsc_conv4", "vhs", "nes", "nes_p0", "nes_p1", "snes", "nesrgb", "nesrgb_p0", "nesrgb_p1", "template", "pv1k", "ntsc_bloom")
+# The NES built with the reference's NES_BORDER 1 (crt_nes.c:64-69): the encoder draws settings.border_color around the
+# picture.  Kept apart from VARIANTS, whose members all encode what the stock build of their system encodes: code that
+# sweeps VARIANTS against a CPU model of the stock encoders would see a border it does not expect.
+BORDER_VARIANTS = ("nes_border", "nes_p0_border")
+ALL_VARIANTS = VARIANTS + BORDER_VARIANTS
 
 
 def lib_path(variant):
@@ -33,14 +38,15 @@ class Source(C.Structure):  # crtx_source
     _fields_ = [("data", C.c_void_p), ("format", C.c_int), ("w", C.c_int), ("h", C.c_int),
                 ("raw", C.c_int), ("as_color", C.c_int), ("field", C.c_int), ("frame", C.c_int),
                 ("hue", C.c_int), ("xoffset", C.c_int), ("yoffset", C.c_int),
-                ("do_aberration", C.c_int), ("dot_crawl_offset", C.c_int), ("reinit", C.c_int), ("pitch", C.c_int)]
+                ("do_aberration", C.c_int), ("dot_crawl_offset", C.c_int), ("reinit", C.c_int), ("pitch", C.c_int),
+                ("border_color", C.c_uint)]  # (read by the NES border builds only)
 
 
 def source_table(sources):
     """numpy structured view (shared memory) of a ctypes array of Source: whole columns of settings can be filled with
     array assignments instead of one Python attribute store per field and monitor (video.VideoConverter)."""
     import numpy as np
-    dt = np.dtype([(n, "u8" if t is C.c_void_p else "i4") for n, t in Source._fields_], align=True)
+    dt = np.dtype([(n, "u8" if t is C.c_void_p else "u4" if t is C.c_uint else "i4") for n, t in Source._fields_], align=True)
     assert dt.itemsize == C.sizeof(Source), (dt.itemsize, C.sizeof(Source))
     return np.frombuffer(sources, dtype=dt)
 
@@ -71,7 +77,7 @@ class Line(C.Structure):  # crtx_line
 
 CRT_EXPORTS = ("crt_init", "crt_resize", "crt_reset", "crt_modulate", "crt_demodulate",
                "crt_bpp4fmt", "crt_sincos14")
-CRTX_EXPORTS = ("crtx_system", "crtx_chroma_pattern", "crtx_hres", "crtx_input_size", "crtx_lines",
+CRTX_EXPORTS = ("crtx_system", "crtx_chroma_pattern", "crtx_nes_border", "crtx_hres", "crtx_input_size", "crtx_lines",
                 "crtx_cc_vper", "crtx_create", "crtx_destroy", "crtx_set_monitors", "crtx_set_state",
                 "crtx_get_state", "crtx_seed", "crtx_analog", "crtx_inp", "crtx_read_signal",
                 "crtx_write_signal", "crtx_modulate",
@@ -118,7 +124,9 @@ def load(variant):
     lib.crtx_set_option.argtypes = [vp, C.c_char_p, ip]
     lib.crtx_get_timing.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_long)]
     lib.crtx_last_error.restype = C.c_char_p
-    assert lib.crtx_system() == spec.system and lib.crtx_hres() == spec.hres, "variant mismatch"
+    lib.crtx_nes_border.restype = ip
+    assert (lib.crtx_system() == spec.system and lib.crtx_hres() == spec.hres
+            and lib.crtx_nes_border() == int(spec.border)), "variant mismatch"
     _libs[variant] = lib
     return lib
 

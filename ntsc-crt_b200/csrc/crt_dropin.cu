@@ -216,6 +216,9 @@ void crt_modulate(struct CRT *v, struct NTSC_SETTINGS *s)
     src.xoffset = s->xoffset;
     src.yoffset = s->yoffset;
     src.dot_crawl_offset = s->dot_crawl_offset;
+#if NES_BORDER
+    src.border_color = s->border_color; /* crt_nes.c:138-161 */
+#endif
     const size_t img_bytes = (size_t) s->w * s->h * sizeof(unsigned short);
 #elif (CRT_SYSTEM == CRT_SYSTEM_NESRGB)
     src.reinit = !s->field_initialized; /* crt_nesrgb.c:63-66: setup_field runs before the format check */

@@ -759,8 +759,36 @@ __global__ void __launch_bounds__(256) k_nes_table(const SrcCfg *__restrict__ sr
     }
 }
 
-// grid (kNesParts, n): each CTA takes every kNesParts-th chunk of the monitor's work
-__global__ void __launch_bounds__(256) k_mod_nes(const SrcCfg *__restrict__ srcs, const signed char *__restrict__ tabs,
+// Border colour (NES_BORDER 1, crt_nes.c:138-161).  Signal line n gets the border when kBorderLo <= n <= kBorderHi;
+// its sample t >= LAV_BEG is the table entry of pixel 0xf0 (at LAV_BEG) or of the border colour, at chroma phase
+// phasetab[(n + dot_crawl_offset) % 3] + 6 + 3 (t - LAV_BEG).  square_sample reads bits 0-8 of the pixel only, so the
+// mask keeps any unsigned border colour exact.
+__device__ __forceinline__ bool nes_border_line(int n) { return kNesBorder && n >= kBorderLo && n <= kBorderHi; }
+// (read where it is used: held in a register across k_mod_nes it takes the kernel past 32 registers, see the pitch below)
+__device__ __forceinline__ unsigned nes_border_color(const SrcCfg *src)
+{
+#if NES_BORDER
+    return __ldg(&src->border_color);
+#else
+    (void) src; // (the record has no border colour in the other builds, which never draw a border)
+    return 0u;
+#endif
+}
+__device__ __forceinline__ signed char nes_border_sample(const signed char *tab, unsigned color, int n, int dot_crawl,
+                                                         int t)
+{
+    const unsigned p = (t == kLavBeg) ? 0xf0u : (color & 0x1ffu);
+    return tab[p * 12 + (((n + dot_crawl) % 3) * 4 + 6 + 3 * (t - kLavBeg)) % 12];
+}
+
+// grid (kNesParts, n): each CTA takes every kNesParts-th chunk of the monitor's work.  The stock build fits 32 registers
+// unasked; the border build is held there, so it keeps 8 CTAs per SM too.
+#if NES_BORDER
+#define CRT_NES_MOD_BOUNDS __launch_bounds__(256, 8)
+#else
+#define CRT_NES_MOD_BOUNDS __launch_bounds__(256)
+#endif
+__global__ void CRT_NES_MOD_BOUNDS k_mod_nes(const SrcCfg *__restrict__ srcs, const signed char *__restrict__ tabs,
                                                  signed char *__restrict__ analog_base, int first)
 {
     __shared__ __align__(16) signed char tab[kNesTabBytes];
@@ -776,7 +804,20 @@ __global__ void __launch_bounds__(256) k_mod_nes(const SrcCfg *__restrict__ srcs
     const signed char *burst = tab + 512 * 12;
 
     // this CTA's share: lines n with n % kNesParts == part (skeleton), picture lines y likewise
-    if (s.reinit) { // setup_field, crt_nes.c:81-104: every line whole; picture lines are done below
+    if constexpr (kNesBorder) {
+        // Lines outside the picture: the skeleton on reinit, and the border -- on every call -- on the border lines.
+        // A thread writes each byte's final value once, so the skeleton under the border is never stored.
+        for (int n = part; n < kVres; n += kNesParts) {
+            if (n >= yo && n < yo + kLines) continue; // written by the CTA that owns the picture line
+            const bool border = nes_border_line(n);
+            if (!s.reinit && !border) continue;
+            const int sync_end = (n >= 259) ? kNesVsyncEnd : kBwBeg;
+            for (int t = (s.reinit ? 0 : kLavBeg) + tid; t < kHres; t += 256)
+                analog[n * kHres + t] = (border && t >= kLavBeg)
+                    ? nes_border_sample(tab, nes_border_color(&srcs[m]), n, s.dot_crawl_offset, t)
+                    : (signed char) ((t >= kSyncBeg && t < sync_end) ? kSync : kBlank);
+        }
+    } else if (s.reinit) { // setup_field, crt_nes.c:81-104: every line whole; picture lines are done below
         for (int n = part; n < kVres; n += kNesParts) {
             if (n >= yo && n < yo + kLines) continue; // written (skeleton first) by the CTA that owns the line
             const int sync_end = (n >= 259) ? kNesVsyncEnd : kBwBeg;
@@ -787,12 +828,23 @@ __global__ void __launch_bounds__(256) k_mod_nes(const SrcCfg *__restrict__ srcs
     const unsigned char *data = static_cast<const unsigned char *>(s.data);
     for (int y = part; y < kLines; y += kNesParts) {
         const int n = y + yo;
-        // every byte of a picture line is written by this one CTA, in order: skeleton, burst, picture
+        // every byte of a picture line is written by this one CTA, in order: skeleton, border, burst, picture
         if (s.reinit) {
             const int sync_end = (n >= 259) ? kNesVsyncEnd : kBwBeg;
-            for (int t = tid; t < kHres; t += 256)
+            // (the border build leaves a border line's bytes from LAV_BEG on to the border and the picture)
+            const int sk_end = nes_border_line(n) ? kLavBeg : kHres;
+            for (int t = tid; t < sk_end; t += 256)
                 analog[n * kHres + t] = (signed char) ((t >= kSyncBeg && t < sync_end) ? kSync : kBlank);
             __syncthreads();
+        }
+        if (nes_border_line(n)) { // the border left of the picture, [LAV_BEG, xo), and right of it, [xo + AV_LEN, HRES)
+            const int left = min(max(xo, kLavBeg), kHres) - kLavBeg;
+            const int r0 = max(xo + kAvLen, kLavBeg);
+            const int right = max(kHres - r0, 0);
+            for (int k = tid; k < left + right; k += 256) {
+                const int t = (k < left) ? kLavBeg + k : r0 + (k - left);
+                analog[n * kHres + t] = nes_border_sample(tab, nes_border_color(&srcs[m]), n, s.dot_crawl_offset, t);
+            }
         }
         if (tid < kBurstLen) { // crt_nes.c:174-178
             const int t = kCbBeg + tid;

@@ -40,6 +40,9 @@ struct SrcCfg { // host -> device, struct NTSC_SETTINGS
     int reinit;
     int compact; // internal (crtx_frames_host): `data` holds only the rows this field reads, picture line y in row y
     int pitch;   // bytes between source rows (resolved by the host: crtx_source's 0 becomes w * bpp, NES w * 2)
+#if NES_BORDER
+    unsigned border_color; // (only in the border build: every other build keeps the record, and its kernels, as they were)
+#endif
 };
 
 typedef crtx_line LineRec; // 32 bytes

@@ -91,6 +91,13 @@ constexpr int kSync = SYNC_LEVEL;
 #if (CRT_SYSTEM == CRT_SYSTEM_NES) || (CRT_SYSTEM == CRT_SYSTEM_NESRGB)
 constexpr int kNesVsyncEnd = PPUpx2pos(327); // crt_nes.c:91, crt_nesrgb.c:33
 #endif
+// NES_BORDER 1 (crt_nes.c:64-69; crt_b200.h): the NES encoder draws the border colour on lines kTop .. kBot + 2 from
+// LAV_BEG on (crt_nes.c:138-161)
+constexpr bool kNesBorder = (NES_BORDER != 0);
+#if (CRT_SYSTEM == CRT_SYSTEM_NES)
+constexpr int kLavBeg = LAV_BEG;
+constexpr int kBorderLo = kTop, kBorderHi = kBot + 2; // (inclusive)
+#endif
 
 // Slack after each signal buffer: the reference reads its decode windows up to one line past
 // inp[] when sync is lost (crt_core.c:438-441,458,511); those reads are outside the parity

@@ -703,6 +703,9 @@ void fill_src(SrcCfg *d, const crtx_source *s)
 #if (CRT_SYSTEM == CRT_SYSTEM_NES)
     d->format = CRT_PIX_FORMAT_RGB; // unused by the NES encoder
 #endif
+#if NES_BORDER
+    d->border_color = s->border_color;
+#endif
 }
 
 // crtx_modulate / crtx_frames_host: the source pitches, all of them before anything is applied
@@ -732,6 +735,7 @@ const char *crtx_last_error(void) { return g_error; }
 
 int crtx_system(void) { return kSystem; }
 int crtx_chroma_pattern(void) { return kPattern; }
+int crtx_nes_border(void) { return kNesBorder ? 1 : 0; }
 int crtx_hres(void) { return kHres; }
 int crtx_input_size(void) { return kInputSize; }
 int crtx_lines(void) { return kLines; }

@@ -27,7 +27,7 @@ def bpp4fmt(fmt):
 
 @dataclass(frozen=True)
 class SystemSpec:
-    name: str          # library suffix: ntsc | ntsc_conv[6|5|4] | vhs | nes | nes_p0 | snes
+    name: str          # library suffix: ntsc | ntsc_conv[6|5|4] | vhs | nes | nes_p0 | nes_border | snes | ...
     system: int        # CRT_SYSTEM
     pattern: int       # CRT_CHROMA_PATTERN
     hres: int
@@ -46,6 +46,7 @@ class SystemSpec:
     burst: int
     black: int
     sync: int
+    border: bool = False  # NES_BORDER 1 (crt_nes.c:64-69): the NES encoder draws settings.border_color
 
     @property
     def input_size(self):
@@ -71,13 +72,13 @@ def _rgb_spec(name, system):
                       8, 8, 100, 20, 7, -40)
 
 
-def _nes_spec(name, pattern):
+def _nes_spec(name, pattern, border=False):
     # crt_nes.h:30-130
     hres = {0: 2280, 1: 2275, 2: 2273}[pattern] * 4 // 10
     p = lambda px: px * hres // 341
     return SystemSpec(name, SYS_NES, pattern, hres, 262, 15, 255, 3,
                       p(9), p(34), p(38), p(74), p(256),
-                      6, 6, 110, 30, 0, -37)
+                      6, 6, 110, 30, 0, -37, border)
 
 
 def _snes_spec(name):
@@ -106,6 +107,9 @@ SPECS = {
     "nes": _nes_spec("nes", 2),
     "nes_p0": _nes_spec("nes_p0", 0),
     "nes_p1": _nes_spec("nes_p1", 1),  # crt_nes.h:33-34: 227.5 cycles per line (the NTSC line length, HRES 910)
+    # NES_BORDER 1 (crt_nes.c:64-69): the stock NES timing, and pattern 0 (HRES 912)
+    "nes_border": _nes_spec("nes_border", 2, border=True),
+    "nes_p0_border": _nes_spec("nes_p0_border", 0, border=True),
     "snes": _snes_spec("snes"),
     "nesrgb": _nesrgb_spec("nesrgb"),
     "nesrgb_p0": _nesrgb_spec("nesrgb_p0", 0),
