@@ -111,10 +111,12 @@ __device__ __forceinline__ void stg_u4(void *p, uint4 v)
 {
     asm volatile("st.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
-// 16-byte asynchronous copy global -> shared with the shared side given as an address
+// 16-byte asynchronous copy global -> shared with the shared side given as an address, for rows that are read 64 bytes
+// at a time from left to right: the L2 fetches the whole aligned 128 bytes around the copy, so the next 64 bytes of the
+// row are already in L2 when they are asked for (one DRAM access per 128 bytes of a row instead of two far apart)
 __device__ __forceinline__ void cp_async_16a(unsigned dst_addr, const void *src)
 {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst_addr), "l"(src) : "memory");
+    asm volatile("cp.async.cg.shared.global.L2::128B [%0], [%1], 16;" ::"r"(dst_addr), "l"(src) : "memory");
 }
 
 // Two-way dot product of 16-bit by 8-bit values with 32-bit accumulate (IDP.2A): a holds two 16-bit values (signed when

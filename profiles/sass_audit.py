@@ -14,7 +14,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "ntsc-crt_b200", "lib")
 
 HOT = {  # variant -> substrings of the kernels worth listing
-    "ntsc": ["k_mod_skeleton_rgb", "k_mod_picture_rgb_stagedILi5ELb1", "6k_syncE", "k_linesILb1ELi1ELi5", "k_linesILb0ELi1ELi5"],
+    "ntsc": ["k_mod_skeleton_rgb", "k_mod_picture_rgb_stagedILi5ELb1", "6k_syncE", "k_lines2ILi1ELi5", "k_lines2ILi0ELi5",
+             "k_linesILb1ELi1ELi5", "k_linesILb0ELi1ELi5"],
     "ntsc_conv": ["k_lines_firILb1ELi1ELi5", "k_lines_firILb0ELi1ELi5"],
     "ntsc_conv4": ["k_lines_firILb1ELi1ELi5"],
     "vhs": ["k_noise_vhs", "6k_syncE"],
