@@ -11,7 +11,13 @@ tests/test_oracle_nes_border.py.
 import numpy as np
 
 import support as S
-from ntsc_crt_b200 import layout
+from ntsc_crt_b200 import capi, layout
+
+BORDER_VARIANTS = list(capi.BORDER_VARIANTS)
+# the largest xoffset that keeps the picture inside its line: xo = (AV_BEG + xoffset) & ~3, xo + AV_LEN <= CRT_HRES
+XMAX = {"nes_border": 30, "nes_p0_border": 34}
+# every 9-bit border colour, and colours with bits above bit 8 (square_sample reads bits 0-8 only)
+COLOURS = list(range(512)) + [0x222, 0x10f0, 0xffffffff]
 
 _LEVEL = (-12042, 0, 34406, 81427, -17203, -8028, 19497, 57342,  # crt_nes.c:26-35
           43581, 75693, 112965, 112965, 26951, 52181, 83721, 83721)

@@ -14,6 +14,8 @@ import ctypes as C
 import hashlib
 import json
 import os
+import struct
+import subprocess
 
 import numpy as np
 
@@ -572,6 +574,182 @@ class ProductEngine(CEngine):
         from ntsc_crt_b200 import capi
         capi.load(variant)  # raises if the library is not built: there is no fallback
         super().__init__(capi.lib_path(variant), variant, outw, outh, fmt, out)
+
+
+# ----------------------------------------------------------------------------------
+# the drop-in interface: the product, the oracle and the reference through the same calls
+# ----------------------------------------------------------------------------------
+
+def trio(variant, outw, outh, fmt=layout.PIX_BGRA, oracle=OracleEngine):
+    """(product, CPU model, reference or None where it is not built), each with an outw x outh monitor;
+    oracle(variant, outw, outh, fmt) makes the CPU model (nes_border_oracle.oracle_engine for the border builds)"""
+    gpu = ProductEngine(variant, outw, outh, fmt)
+    ora = oracle(variant, outw, outh, fmt)
+    ref = RefEngine(variant, outw, outh, fmt, seed=1) if have_ref(variant) else None
+    return gpu, ora, ref
+
+
+def run_all(engines, fn):
+    for e in engines:
+        if e is not None:
+            fn(e)
+
+
+def check(gpu, ora, ref, what):
+    assert_same_state(gpu.state(), ora.state(), what + " [gpu vs oracle]")
+    if ref is not None:
+        assert_same_state(gpu.state(), ref.state(), what + " [gpu vs reference]")
+
+
+# ----------------------------------------------------------------------------------
+# the batch interface against one CPU model per monitor
+# ----------------------------------------------------------------------------------
+
+def monitor_state(batch, i, out):
+    """monitor i of a capi.Batch, whose output image is the tensor `out`, as the dict OracleEngine.state() returns"""
+    import torch
+    torch.cuda.synchronize()
+    spec = batch.spec
+    st = batch.get_state(first=i, count=1)[0]
+    return dict(analog=batch.signal(i, "analog"), inp=batch.signal(i, "inp"), out=out.cpu().numpy().copy(),
+                ccf=np.array([[st.ccf[r][x] for x in range(spec.cc_samples)] for r in range(spec.vper)]),
+                hsync=st.hsync, vsync=st.vsync, rn=st.rn)
+
+
+class BatchRig:
+    """A capi.Batch and one CPU model per monitor, driven through the same calls and compared whole state by whole state.
+
+    mons[i] = dict(outw, outh, fmt, noise, knobs), and optionally seed: the VHS rand() seed of both sides.  options:
+    (name, value) pairs set on the batch first.  oracle(variant, outw, outh, fmt, seed=...) makes one monitor's CPU
+    model (nes_border_oracle.oracle_engine for the border builds)."""
+
+    def __init__(self, variant, mons, options=(), oracle=OracleEngine):
+        import torch
+        from ntsc_crt_b200 import capi
+        self.mons = mons
+        self.b = capi.Batch(variant, len(mons))
+        for name, value in options:
+            self.b.set_option(name, value)
+        self.outs, self.oras, self._dev, self._src = [], [], {}, {}
+        for i, m in enumerate(mons):
+            out = torch.zeros(m["outh"], m["outw"], max(1, layout.bpp4fmt(m["fmt"])), dtype=torch.uint8, device="cuda")
+            self.b.set_monitor(i, out, fmt=m["fmt"], noise=m["noise"], **m["knobs"])
+            if "seed" in m:
+                self.b.seed(m["seed"], first=i, count=1)
+            o = oracle(variant, m["outw"], m["outh"], m["fmt"], seed=m.get("seed", 1))
+            o.set(**m["knobs"])
+            self.outs.append(out)
+            self.oras.append(o)
+        self.b.commit_monitors()
+
+    def _device(self, img):
+        import torch
+        if id(img) not in self._dev:  # (the entry keeps img alive, so its id is not reused)
+            dev = torch.from_numpy(img.view(np.int16) if img.dtype == np.uint16 else img).cuda()
+            self._dev[id(img)] = (img, dev)
+        return self._dev[id(img)][1]
+
+    def source(self, i, img, **settings):
+        """monitor i's next source image (numpy) and settings, on both sides.  The batch's `reinit` is the NES and NES-RGB
+        oracles' field_initialized = not reinit; the other oracles have no such setting."""
+        kw = dict(settings)
+        reinit = kw.pop("reinit", None)
+        if reinit is not None and self.b.spec.system in (layout.SYS_NES, layout.SYS_NESRGB):
+            kw["field_initialized"] = int(not reinit)
+        self.b.set_source(i, self._device(img), **settings)
+        self._src[i] = (img, kw)
+
+    def modulate(self, first=0, count=None):
+        count = len(self.mons) - first if count is None else count
+        self.b.modulate(first=first, count=count)
+        for i in range(first, first + count):
+            img, kw = self._src[i]
+            self.oras[i].modulate(img, **kw)
+
+    def demodulate(self, first=0, count=None):
+        count = len(self.mons) - first if count is None else count
+        self.b.demodulate(first=first, count=count)
+        for i in range(first, first + count):
+            self.oras[i].demodulate(self.mons[i]["noise"])
+
+    def seed(self, seed, first, count):
+        self.b.seed(seed, first=first, count=count)
+        for i in range(first, first + count):
+            self.oras[i].lib.ocrt_rand_seed(C.byref(self.oras[i].rand), seed)
+            self.mons[i]["seed"] = seed
+
+    def frames_host(self, host_ptrs):
+        """crtx_frames_host on every monitor: the sources of the last source() calls read from their HOST images, the
+        decoded images copied to host_ptrs[i]"""
+        for i, o in enumerate(self.oras):
+            img, kw = self._src[i]
+            self.b.sources[i].data = img.ctypes.data
+            o.modulate(img, **kw)
+            o.demodulate(self.mons[i]["noise"])
+        self.b.frames_host(host_ptrs)
+
+    def check(self, what):
+        for i, o in enumerate(self.oras):
+            assert_same_state(monitor_state(self.b, i, self.outs[i]), o.state(), "%s, monitor %d %r" % (what, i, self.mons[i]))
+
+    def close(self):
+        self.b.close()
+
+
+# ----------------------------------------------------------------------------------
+# image files, as the reference's drivers read and write them
+# ----------------------------------------------------------------------------------
+
+def write_ppm(path, rgb, maxc=255, comment=False):
+    with open(path, "wb") as f:
+        f.write(b"P6\n" + (b"# made by a test\n" if comment else b"") + b"%d %d\n%d\n" % (rgb.shape[1], rgb.shape[0], maxc))
+        f.write(rgb.tobytes())
+
+
+def write_bmp(path, bgra, bits):
+    """24- or 32-bit bottom-up BMP, rows padded to 4 bytes, as ffmpeg would hand it to the reference's reader"""
+    h, w = bgra.shape[:2]
+    bpp = bits // 8
+    pad = (4 - (w * bpp) % 4) % 4
+    rows = b"".join(bgra[y, :, :bpp].tobytes() + b"\0" * pad for y in range(h - 1, -1, -1))
+    head = b"BM" + struct.pack("<IHHI", 54 + len(rows), 0, 0, 54) + struct.pack("<IiiHHIIiiII", 40, w, h, 1, bits, 0, len(rows), 0, 0, 0, 0)
+    with open(path, "wb") as f:
+        f.write(head + rows)
+
+
+def read_bmp32(path):
+    """a 32-bit BMP as the drivers write it (bmp_rw.c:96-146): 54-byte header, no padding, file size in the header"""
+    raw = open(path, "rb").read()
+    w, h = struct.unpack_from("<ii", raw, 18)
+    bpp = struct.unpack_from("<H", raw, 28)[0]
+    assert raw[:2] == b"BM" and bpp == 32 and struct.unpack_from("<I", raw, 10)[0] == 54
+    assert len(raw) == 54 + w * h * 4 and struct.unpack_from("<I", raw, 2)[0] == len(raw)
+    return np.frombuffer(raw, dtype=np.uint8, offset=54).reshape(h, w, 4)[::-1]
+
+
+def moving_bars(n, w, h, seed=0):
+    """n BGRA frames: colour bars moving right, every frame with its own noise"""
+    rng = np.random.default_rng(seed)
+    base = bars_image(w, h)
+    frames = []
+    for k in range(n):
+        f = np.roll(base, 7 * k, axis=1).copy()
+        f[..., :3] ^= rng.integers(0, 16, size=(h, w, 3), dtype=np.uint8)
+        f[..., 3] = 255  # what the reader makes of 24-bit files (bmp_rw.c:90)
+        frames.append(f)
+    return np.stack(frames)
+
+
+def run_video_convert(exe, where, frames, flags, outw, outh, noise, bits=24):
+    """a build of the reference's extra/video_convert.c on `frames` written as BMP files under `where`: its output files"""
+    os.makedirs(os.path.join(where, "frames"))
+    os.makedirs(os.path.join(where, "output"))
+    for k in range(len(frames)):
+        write_bmp(os.path.join(where, "frames", "%06d.bmp" % (k + 1)), frames[k], bits)
+    # video_convert.c:244: `while (err < nframes)` from 1 -- num_frames - 1 images are converted
+    subprocess.run([exe, flags, str(len(frames) + 1), str(outw), str(outh), str(noise)], cwd=where, check=True,
+                   stdout=subprocess.DEVNULL, timeout=600)
+    return [open(os.path.join(where, "output", "%06d.bmp" % (k + 1)), "rb").read() for k in range(len(frames))]
 
 
 def diff_report(name, x, y, shape_hint=None):

@@ -91,22 +91,13 @@ def test_frames_host_is_the_same_field_with_host_buffers(variant, host_src):
     the copies happen inside the call on the caller's stream.  Images of different sizes (the staging slots grow),
     several fields, outputs compared with the oracle's."""
     import torch
-    from ntsc_crt_b200 import capi
     n = 3
-    b = capi.Batch(variant, n)
-    if host_src:  # "host_src": page-locked source images are read in place by the encoder instead of being copied first
-        b.set_option("host_src", 1)
     nes = variant == "nes"
-    outs = [torch.zeros(480, 640, 4, dtype=torch.uint8, device="cuda") for _ in range(n)]
+    # "host_src": page-locked source images are read in place by the encoder instead of being copied first
+    rig = S.BatchRig(variant, [dict(outw=640, outh=480, fmt=layout.PIX_BGRA, noise=2 * i, knobs=dict(blend=1, scanlines=1))
+                               for i in range(n)], options=(("host_src", 1),) if host_src else ())
     host_outs = [np.zeros((480, 640, 4), dtype=np.uint8) for _ in range(n)]
     pinned = []  # keeps page-locked copies alive
-    oras = []
-    for i in range(n):
-        b.set_monitor(i, outs[i], fmt=layout.PIX_BGRA, noise=2 * i, blend=1, scanlines=1)
-        o = S.OracleEngine(variant, 640, 480)
-        o.set(blend=1, scanlines=1)
-        oras.append(o)
-    b.commit_monitors()
     for it in range(3):
         imgs = [S.nes_image(seed=40 + i + it) if nes else S.rand_image(200 + 150 * i + 64 * it, 120 + 100 * i, seed=40 + i + it)
                 for i in range(n)]
@@ -117,21 +108,13 @@ def test_frames_host_is_the_same_field_with_host_buffers(variant, host_src):
         for i in range(n):
             kw = dict(dot_crawl_offset=it % 3, hue=10 * i) if nes else dict(format=layout.PIX_BGRA, as_color=1, field=it & 1, frame=0,
                                                                               dot_crawl_offset=it % 3)
-            b.sources[i].reinit = 1 if (nes and it == 0) else 0
-            # a HOST image this time: set_source only records the pointer and the size
-            b.sources[i].data = imgs[i].ctypes.data
-            b.sources[i].h, b.sources[i].w = imgs[i].shape[0], imgs[i].shape[1]
-            for k, v in kw.items():
-                setattr(b.sources[i], k, v)
-            oras[i].modulate(imgs[i], **kw)
-            oras[i].demodulate(2 * i)
-        b.frames_host([h.ctypes.data for h in host_outs])
-        torch.cuda.synchronize()
+            rig.source(i, imgs[i], reinit=int(nes and it == 0), **kw)
+        rig.frames_host([h.ctypes.data for h in host_outs])  # HOST source images in, HOST images out
+        rig.check("%s field %d" % (variant, it))
         for i in range(n):
-            assert np.array_equal(host_outs[i], oras[i].out), "%s field %d monitor %d: %s" % (
-                variant, it, i, S.diff_report("host image", host_outs[i], oras[i].out))
-            assert np.array_equal(outs[i].cpu().numpy(), oras[i].out)
-    b.close()
+            assert np.array_equal(host_outs[i], rig.oras[i].out), "%s field %d monitor %d: %s" % (
+                variant, it, i, S.diff_report("host image", host_outs[i], rig.oras[i].out))
+    rig.close()
 
 
 @pytest.mark.parametrize("variant,raw", [("ntsc", 0), ("ntsc", 1), ("pv1k", 0), ("nes", 0), ("ntsc_conv", 0)])

@@ -6,7 +6,7 @@ import pytest
 
 import support as S
 from ntsc_crt_b200 import layout
-from test_gpu_parity import check, run_all, trio
+from support import check, run_all, trio
 
 pytestmark = pytest.mark.gpu
 
@@ -42,38 +42,3 @@ def test_dropin_bloom_formats_and_geometries(fmt, outw, outh, blend, scanlines):
     run_all((gpu, ora, ref), lambda e: e.set(saturation=900, brightness=5000))
     run_all((gpu, ora, ref), lambda e: e.demodulate(3))
     check(gpu, ora, ref, "bloom extreme knobs")
-
-
-def test_batch_bloom_matches_oracle():
-    import torch
-    from ntsc_crt_b200 import capi
-    n = 4
-    b = capi.Batch("ntsc_bloom", n)
-    outs, oras, imgs = [], [], []
-    for i in range(n):
-        t = torch.zeros(480, 640, 4, dtype=torch.uint8, device="cuda")
-        outs.append(t)
-        b.set_monitor(i, t, fmt=layout.PIX_BGRA, noise=20 * i, blend=i & 1, scanlines=1 - (i >> 1), contrast=170 + 10 * i)
-        o = S.OracleEngine("ntsc_bloom", 640, 480)
-        o.set(blend=i & 1, scanlines=1 - (i >> 1), contrast=170 + 10 * i)
-        oras.append(o)
-        imgs.append(S.rand_image(256 + 32 * i, 224, seed=400 + i) if i else np.full((200, 300, 4), 250, dtype=np.uint8))
-    b.commit_monitors()
-    dimgs = [torch.from_numpy(im).cuda() for im in imgs]
-    for it in range(4):
-        for i in range(n):
-            kw = dict(format=layout.PIX_BGRA, as_color=1, hue=15 * i, field=it & 1, frame=(it >> 1) & 1)
-            b.set_source(i, dimgs[i], **kw)
-            oras[i].modulate(imgs[i], **kw)
-            oras[i].demodulate(20 * i)
-        b.modulate()
-        b.demodulate()
-        torch.cuda.synchronize()
-        st = b.get_state()
-        for i in range(n):
-            got = outs[i].cpu().numpy()
-            assert np.array_equal(got, oras[i].out), "bloom batch monitor %d field %d: %s" % (
-                i, it, S.diff_report("out", got, oras[i].out))
-            assert np.array_equal(b.signal(i, "inp"), oras[i].inp), (i, it)
-            assert (st[i].hsync, st[i].vsync, st[i].rn) == (oras[i].hsync, oras[i].vsync, oras[i].rn), (i, it)
-    b.close()

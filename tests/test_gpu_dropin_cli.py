@@ -16,18 +16,12 @@ REF_CLI = os.path.join(S.REF_DIR, "cli_ref_ntsc")
 B200_CLI = os.path.join(S.REF_DIR, "cli_b200_ntsc")
 
 
-def write_ppm(path, rgb):
-    with open(path, "wb") as f:
-        f.write(b"P6\n%d %d\n255\n" % (rgb.shape[1], rgb.shape[0]))
-        f.write(rgb.tobytes())
-
-
 @pytest.mark.skipif(not (os.path.exists(REF_CLI) and os.path.exists(B200_CLI)), reason="driver binaries not built")
 @pytest.mark.parametrize("flags,noise,hue", [("-op", 0, 0), ("-o", 12, 0), ("-om", 24, 30), ("-opr", 0, 90), ("-opa", 0, 0)])
 def test_unmodified_cli_driver_is_byte_identical(tmp_path, flags, noise, hue):
     rgb = S.bars_image(320, 240, fmt=S.layout.PIX_RGB)[..., :3].copy()
     src = tmp_path / "in.ppm"
-    write_ppm(str(src), rgb)
+    S.write_ppm(str(src), rgb)
     outs = []
     for exe, name in ((REF_CLI, "ref.ppm"), (B200_CLI, "b200.ppm")):
         out = tmp_path / name
@@ -49,7 +43,7 @@ def test_unmodified_cli_driver_other_systems(tmp_path, system, flags, noise, hue
         pytest.skip("driver binaries not built")
     rgb = S.bars_image(320, 240, fmt=S.layout.PIX_RGB)[..., :3].copy()
     src = tmp_path / "in.ppm"
-    write_ppm(str(src), rgb)
+    S.write_ppm(str(src), rgb)
     outs = []
     for exe, name in ((ref_cli, "ref.ppm"), (b200_cli, "b200.ppm")):
         out = tmp_path / name

@@ -5,7 +5,7 @@ import pytest
 
 import support as S
 from ntsc_crt_b200 import layout
-from test_gpu_parity import check, run_all, trio
+from support import check, run_all, trio
 
 pytestmark = pytest.mark.gpu
 

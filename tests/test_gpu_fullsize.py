@@ -2,8 +2,7 @@
 interlaced, blend 1, scanlines 1 -- checked through a size-independent property instead of 264 oracle runs: monitors
 that are fed the same image, settings and noise must stay bit-identical to each other through every field (a checksum
 of checksums: one representative per group against all its members, on the device), and the representatives are
-compared with the oracle.  Also: the context's state after the run equals the oracle's for every monitor."""
-import numpy as np
+compared with the oracle, whole state.  Also: the context's whole state after the run equals the oracle's for every monitor."""
 import pytest
 
 import support as S
@@ -47,14 +46,8 @@ def test_full_size_batch_is_consistent_and_matches_the_oracle():
             same = (members == members[0:1]).reshape(members.shape[0], -1).all(dim=1)
             assert bool(same.all()), "field %d group %d: monitors %r differ from monitor %d" % (
                 it, g, [g + GROUPS * int(k) for k in torch.nonzero(~same).flatten()[:8]], g)
-            got = outs[g].cpu().numpy()
-            assert np.array_equal(got, oras[g].out), "field %d group %d: %s" % (it, g, S.diff_report("out", got, oras[g].out))
-    st = b.get_state()
+            S.assert_same_state(S.monitor_state(b, g, outs[g]), oras[g].state(), "field %d group %d" % (it, g))
+    want = [o.state() for o in oras]
     for i in range(n):
-        o = oras[i % GROUPS]
-        assert (st[i].hsync, st[i].vsync, st[i].rn) == (o.hsync, o.vsync, o.rn), i
-        assert [st[i].ccf[0][x] for x in range(4)] == o.ccf[0].tolist(), i
-    for g in range(GROUPS):  # the signal buffers of the last monitor of each group
-        i = g + GROUPS * ((n - 1 - g) // GROUPS)
-        assert np.array_equal(b.signal(i, "analog"), oras[g].analog) and np.array_equal(b.signal(i, "inp"), oras[g].inp), i
+        S.assert_same_state(S.monitor_state(b, i, outs[i]), want[i % GROUPS], "monitor %d after the run" % i)
     b.close()

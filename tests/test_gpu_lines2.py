@@ -1,7 +1,7 @@
 """k_lines2 (csrc/crt_lines2.cuh): the line pass the common geometries take -- two monitors per CTA, tabulated
 resampler, ring of decoded samples.  Every case runs the batch interface twice, with the kernel on (and proven to
 have been taken: crtx_lines2_count) and with `lines2` off (k_lines), and compares both with the oracle after every
-field: image, hsync / vsync / rn.  Geometries at and beyond the kernel's limits, every 4-byte pixel format, odd
+field: the whole state.  Geometries at and beyond the kernel's limits, every 4-byte pixel format, odd
 monitor counts (a CTA with one monitor), scanline-block windows, knobs that move the luma bias, and a batch in which
 one monitor of a CTA's pair needs the wrap-exact equaliser (it must be left to k_lines<generic>)."""
 import numpy as np
@@ -17,52 +17,27 @@ FMT4 = (layout.PIX_ARGB, layout.PIX_RGBA, layout.PIX_ABGR, layout.PIX_BGRA)
 
 def _run(variant, outw, outh, n, fields, fmt=layout.PIX_BGRA, noise=0, expect_lines2=True, options=(), knobs=None,
          per_monitor_knobs=None, src=(256, 240), line_window=None):
-    import torch
-    from ntsc_crt_b200 import capi
-    knobs = dict(knobs or {})
+    options = tuple(options) + ((("line_lo", line_window[0]), ("line_hi", line_window[1])) if line_window else ())
+    mons = [dict(outw=outw, outh=outh, fmt=fmt, noise=noise + i, knobs=dict(knobs or {}, **(per_monitor_knobs or {}).get(i, {})))
+            for i in range(n)]
+    imgs = [S.rand_image(src[0], src[1], seed=70 + i) for i in range(n)]
     results = {}
     for lines2 in (1, 0):
-        b = capi.Batch(variant, n)
-        b.set_option("lines2", lines2)
-        for name, val in options:
-            b.set_option(name, val)
-        if line_window:
-            b.set_option("line_lo", line_window[0])
-            b.set_option("line_hi", line_window[1])
-        outs = [torch.zeros(outh, outw, 4, dtype=torch.uint8, device="cuda") for _ in range(n)]
-        imgs = [S.rand_image(src[0], src[1], seed=70 + i) for i in range(n)]
-        dimgs = [torch.from_numpy(im).cuda() for im in imgs]
-        oras = []
-        for i in range(n):
-            k = dict(knobs)
-            k.update((per_monitor_knobs or {}).get(i, {}))
-            b.set_monitor(i, outs[i], fmt=fmt, noise=noise + i, **k)
-            o = S.OracleEngine(variant, outw, outh, fmt=fmt)
-            o.set(**k)
-            oras.append(o)
-        b.commit_monitors()
+        rig = S.BatchRig(variant, mons, options=(("lines2", lines2),) + options)
         for f in range(fields):
             for i in range(n):
-                b.set_source(i, dimgs[i], format=layout.PIX_BGRA, as_color=1, field=f & 1, frame=(f >> 1) & 1)
-            b.modulate()
-            b.demodulate()
-            torch.cuda.synchronize()
-            st = b.get_state()
-            for i in range(n):
-                if line_window is None:
-                    oras[i].modulate(imgs[i], format=layout.PIX_BGRA, as_color=1, field=f & 1, frame=(f >> 1) & 1)
-                    oras[i].demodulate(noise + i)
-                    got = outs[i].cpu().numpy()
-                    assert np.array_equal(got, oras[i].out), "lines2=%d field %d monitor %d: %s" % (
-                        lines2, f, i, S.diff_report("image", got, oras[i].out))
-                    assert (st[i].hsync, st[i].vsync, st[i].rn) == (oras[i].hsync, oras[i].vsync, oras[i].rn)
-        took = b.lines2_launches
+                rig.source(i, imgs[i], format=layout.PIX_BGRA, as_color=1, field=f & 1, frame=(f >> 1) & 1)
+            rig.modulate()
+            rig.demodulate()
+            if line_window is None:
+                rig.check("lines2=%d field %d" % (lines2, f))
+        took = rig.b.lines2_launches
         if lines2 == 1:
             assert (took > 0) == expect_lines2, "k_lines2 launches: %d (expected %s)" % (took, expect_lines2)
         else:
             assert took == 0
-        results[lines2] = [o.cpu().numpy().copy() for o in outs]
-        b.close()
+        results[lines2] = [o.cpu().numpy().copy() for o in rig.outs]
+        rig.close()
     for i in range(n):  # the two kernels agree bit for bit (this is the whole check for the scanline-window case)
         assert np.array_equal(results[1][i], results[0][i]), "monitor %d: %s" % (i, S.diff_report("k_lines2 vs k_lines", results[1][i], results[0][i]))
     return results
@@ -127,24 +102,13 @@ def test_scanline_window():
 @pytest.mark.parametrize("variant", ["vhs", "template", "nes", "snes", "nesrgb"])
 def test_other_systems_take_it_too(variant):
     """every build with four samples per chroma period and the IIR equaliser has the kernel"""
-    import torch
-    from ntsc_crt_b200 import capi
     n, outw, outh = 3, 832, 624
     nes = variant == "nes"
+    imgs = [S.nes_image(seed=5 + i) if nes else S.rand_image(256, 240, seed=5 + i) for i in range(n)]
     res = {}
     for lines2 in (1, 0):
-        b = capi.Batch(variant, n)
-        b.set_option("lines2", lines2)
-        outs = [torch.zeros(outh, outw, 4, dtype=torch.uint8, device="cuda") for _ in range(n)]
-        oras = []
-        for i in range(n):
-            b.set_monitor(i, outs[i], fmt=layout.PIX_BGRA, noise=2 + i, blend=1, scanlines=1)
-            o = S.OracleEngine(variant, outw, outh)
-            o.set(blend=1, scanlines=1)
-            oras.append(o)
-        b.commit_monitors()
-        imgs = [S.nes_image(seed=5 + i) if nes else S.rand_image(256, 240, seed=5 + i) for i in range(n)]
-        dimgs = [torch.from_numpy(im.astype(np.int16) if nes else im).cuda() for im in imgs]
+        rig = S.BatchRig(variant, [dict(outw=outw, outh=outh, fmt=layout.PIX_BGRA, noise=2 + i, knobs=dict(blend=1, scanlines=1))
+                                   for i in range(n)], options=(("lines2", lines2),))
         for f in range(3):
             for i in range(n):
                 if nes:
@@ -153,20 +117,13 @@ def test_other_systems_take_it_too(variant):
                     kw = dict(format=layout.PIX_BGRA, dot_crawl_offset=f % 3, hue=0)
                 else:
                     kw = dict(format=layout.PIX_BGRA, as_color=1, field=f & 1, frame=0, dot_crawl_offset=f % 3)
-                b.sources[i].reinit = 1 if f == 0 else 0
-                b.set_source(i, dimgs[i], **kw)
-                oras[i].modulate(imgs[i], **kw)
-                oras[i].demodulate(2 + i)
-            b.modulate()
-            b.demodulate()
-            torch.cuda.synchronize()
-            for i in range(n):
-                got = outs[i].cpu().numpy()
-                assert np.array_equal(got, oras[i].out), "%s lines2=%d field %d monitor %d: %s" % (
-                    variant, lines2, f, i, S.diff_report("image", got, oras[i].out))
-        assert (b.lines2_launches > 0) == (lines2 == 1)
-        res[lines2] = [o.cpu().numpy().copy() for o in outs]
-        b.close()
+                rig.source(i, imgs[i], reinit=int(f == 0), **kw)
+            rig.modulate()
+            rig.demodulate()
+            rig.check("%s lines2=%d field %d" % (variant, lines2, f))
+        assert (rig.b.lines2_launches > 0) == (lines2 == 1)
+        res[lines2] = [o.cpu().numpy().copy() for o in rig.outs]
+        rig.close()
     for i in range(n):
         assert np.array_equal(res[1][i], res[0][i])
 

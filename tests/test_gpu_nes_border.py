@@ -11,16 +11,11 @@ import numpy as np
 import pytest
 
 import support as S
-from nes_border_oracle import oracle_engine
+from nes_border_oracle import BORDER_VARIANTS, COLOURS, XMAX, oracle_engine
 from ntsc_crt_b200 import capi, layout, sharding
 from test_simt_kernels import simt_libs  # noqa: F401  (session fixture of the interpreter builds)
 import test_simt_kernels as _simt
 
-BORDER_VARIANTS = list(capi.BORDER_VARIANTS)
-# the largest xoffset that keeps the picture inside its line: xo = (AV_BEG + xoffset) & ~3, xo + AV_LEN <= CRT_HRES
-XMAX = {"nes_border": 30, "nes_p0_border": 34}
-# every 9-bit border colour, and colours with bits above bit 8 (square_sample reads bits 0-8 only)
-COLOURS = list(range(512)) + [0x222, 0x10f0, 0xffffffff]
 # monitor knobs: (black_point, white_point, hue, blend, scanlines)
 KNOBS = [(0, 100, 0, 1, 1), (6, 90, 20, 0, 1), (-4, 115, -30, 1, 0), (12, 80, 75, 0, 0)]
 
@@ -28,12 +23,8 @@ BATCH, FIELDS = 64, 9  # every colour in COLOURS at least once across the batch'
 OUTW, OUTH = 400, 300
 
 
-def _xmax(variant):
-    return XMAX[variant]
-
-
 def _settings(variant, it, i, n):
-    return dict(dot_crawl_offset=(i + it) % 3, hue=(37 * i + 11 * it) % 360, xoffset=(7 * i + 3 * it) % (_xmax(variant) + 1),
+    return dict(dot_crawl_offset=(i + it) % 3, hue=(37 * i + 11 * it) % 360, xoffset=(7 * i + 3 * it) % (XMAX[variant] + 1),
                 yoffset=(i + it) % 8, border_color=COLOURS[(it * n + i) % len(COLOURS)])
 
 
@@ -42,108 +33,69 @@ def _reinit(it, i):
     return it == 0 or (it == 3 and i % 2 == 1)
 
 
-def _compare_monitor(b, st, i, o, what):
-    got = b.signal(i, "analog")
-    assert np.array_equal(got, o.analog), "%s analog: %s" % (what, S.diff_report("analog", got, o.analog))
-    got = b.signal(i, "inp")
-    assert np.array_equal(got, o.inp), "%s inp: %s" % (what, S.diff_report("inp", got, o.inp))
-    ccf = np.array([[st[i].ccf[r][x] for x in range(4)] for r in range(3)])
-    assert np.array_equal(ccf, o.ccf), (what, ccf, o.ccf)
-    assert (st[i].hsync, st[i].vsync, st[i].rn) == (o.hsync, o.vsync, o.rn), what
-
-
 def check_batch(variant, n=None, fields=None):
-    """n monitors for `fields` consecutive fields, every field's analog, inp, out, ccf, hsync and vsync against the oracle"""
-    import torch
+    """n monitors for `fields` consecutive fields, every field's whole state against the oracle"""
     n, fields = n or BATCH, fields or FIELDS
-    b = capi.Batch(variant, n)
-    outs, oras, imgs = [], [], []
+    mons = []
     for i in range(n):
         bp, wp, hue, blend, scan = KNOBS[i % len(KNOBS)]
-        t = torch.zeros(OUTH, OUTW, 4, dtype=torch.uint8, device="cuda")
-        outs.append(t)
-        b.set_monitor(i, t, fmt=layout.PIX_BGRA, noise=(5 * i) % 17, blend=blend, scanlines=scan, black_point=bp,
-                      white_point=wp, hue=hue)
-        o = oracle_engine(variant, OUTW, OUTH)
-        o.set(blend=blend, scanlines=scan, black_point=bp, white_point=wp, hue=hue)
-        oras.append(o)
-        imgs.append(S.nes_image(seed=300 + i, rainbow=(i % 5 == 4)))
-    b.commit_monitors()
-    dimgs = [torch.from_numpy(im.astype(np.int16)).cuda() for im in imgs]
+        mons.append(dict(outw=OUTW, outh=OUTH, fmt=layout.PIX_BGRA, noise=(5 * i) % 17,
+                         knobs=dict(blend=blend, scanlines=scan, black_point=bp, white_point=wp, hue=hue)))
+    rig = S.BatchRig(variant, mons, oracle=oracle_engine)
+    imgs = [S.nes_image(seed=300 + i, rainbow=(i % 5 == 4)) for i in range(n)]
     for it in range(fields):
         for i in range(n):
-            kw = _settings(variant, it, i, n)
-            b.set_source(i, dimgs[i], **kw)
-            b.sources[i].reinit = int(_reinit(it, i))
-            oras[i].modulate(imgs[i], field_initialized=int(not _reinit(it, i)), **kw)
-            oras[i].demodulate((5 * i) % 17)
-        b.modulate()
-        b.demodulate()
-        torch.cuda.synchronize()
-        st = b.get_state()
-        for i in range(n):
-            what = "%s field %d monitor %d" % (variant, it, i)
-            got = outs[i].cpu().numpy()
-            assert np.array_equal(got, oras[i].out), "%s: %s" % (what, S.diff_report("out", got, oras[i].out))
-            _compare_monitor(b, st, i, oras[i], what)
-    b.close()
+            rig.source(i, imgs[i], reinit=int(_reinit(it, i)), **_settings(variant, it, i, n))
+        rig.modulate()
+        rig.demodulate()
+        rig.check("%s field %d" % (variant, it))
+    rig.close()
 
 
 def check_dropin(variant, fields=8):
     """the drop-in interface (crt_modulate / crt_demodulate, NTSC_SETTINGS.border_color), after every call; the settings
     are re-initialised once more half way"""
-    from test_gpu_parity import check, run_all
-    gpu = S.ProductEngine(variant, 832, 624)
-    ora = oracle_engine(variant, 832, 624)
-    ref = S.RefEngine(variant, 832, 624, seed=1) if S.have_ref(variant) else None
-    run_all((gpu, ora, ref), lambda e: e.set(blend=1, scanlines=1, black_point=3, white_point=93))
+    gpu, ora, ref = S.trio(variant, 832, 624, oracle=oracle_engine)
+    S.run_all((gpu, ora, ref), lambda e: e.set(blend=1, scanlines=1, black_point=3, white_point=93))
     img = S.nes_image(seed=21)
     for it in range(fields):
         kw = dict(border_color=[0x22, 0x0f, 0x1ff, 0x2d, 0x30, 0x100 | 0x16, 0x0d, 0x222][it % 8], dot_crawl_offset=it % 3,
-                  hue=(it * 40) % 360, xoffset=[0, _xmax(variant), 16, 7, 3, 28, 12, 1][it % 8], yoffset=it % 8)
+                  hue=(it * 40) % 360, xoffset=[0, XMAX[variant], 16, 7, 3, 28, 12, 1][it % 8], yoffset=it % 8)
         if it == fields // 2:
             kw["field_initialized"] = 0
-        run_all((gpu, ora, ref), lambda e: e.modulate(img, **kw))
-        check(gpu, ora, ref, "%s drop-in mod %d" % (variant, it))
-        run_all((gpu, ora, ref), lambda e: e.demodulate(3 * it))
-        check(gpu, ora, ref, "%s drop-in demod %d" % (variant, it))
+        S.run_all((gpu, ora, ref), lambda e: e.modulate(img, **kw))
+        S.check(gpu, ora, ref, "%s drop-in mod %d" % (variant, it))
+        S.run_all((gpu, ora, ref), lambda e: e.demodulate(3 * it))
+        S.check(gpu, ora, ref, "%s drop-in demod %d" % (variant, it))
 
 
 def check_frames_host(variant, n=3, fields=4):
-    """crtx_frames_host: host source images in, host images out; the output rows the fields write equal the oracle's"""
+    """crtx_frames_host: host source images in, host images out; the whole state, and the output rows the fields write
+    in the host images, equal the oracle's"""
     import torch
     outw, outh = 640, 480
-    b = capi.Batch(variant, n)
-    outs = [torch.zeros(outh, outw, 4, dtype=torch.uint8, device="cuda") for _ in range(n)]
+    rig = S.BatchRig(variant, [dict(outw=outw, outh=outh, fmt=layout.PIX_BGRA, noise=2 + i,
+                                    knobs=dict(blend=1, scanlines=1, black_point=i, white_point=100 - 5 * i)) for i in range(n)],
+                     oracle=oracle_engine)
     host = [torch.zeros(outh, outw, 4, dtype=torch.uint8).pin_memory() for _ in range(n)]
-    oras = []
-    for i in range(n):
-        b.set_monitor(i, outs[i], fmt=layout.PIX_BGRA, noise=2 + i, blend=1, scanlines=1, black_point=i, white_point=100 - 5 * i)
-        o = oracle_engine(variant, outw, outh)
-        o.set(blend=1, scanlines=1, black_point=i, white_point=100 - 5 * i)
-        oras.append(o)
-    b.commit_monitors()
     srcs = [torch.from_numpy(S.nes_image(256, 240 - 16 * i, seed=60 + i).astype(np.int16)).pin_memory() for i in range(n)]
+    imgs = [s.numpy().view(np.uint16) for s in srcs]  # (the page-locked images themselves)
     for it in range(fields):
         for i in range(n):
-            kw = dict(dot_crawl_offset=(it + i) % 3, hue=15 * i, xoffset=(9 * it + 5 * i) % (_xmax(variant) + 1),
-                      yoffset=(it + 2 * i) % 8, border_color=(0x22 + 0x41 * it + 0x9 * i) & 0x1ff)
-            b.set_source(i, srcs[i], **kw)
-            b.sources[i].reinit = int(it == 0)
-            oras[i].modulate(srcs[i].numpy().view(np.uint16), field_initialized=int(it != 0), **kw)
-            oras[i].demodulate(2 + i)
-        b.frames_host([h.data_ptr() for h in host])
-        torch.cuda.synchronize()
+            rig.source(i, imgs[i], reinit=int(it == 0), dot_crawl_offset=(it + i) % 3, hue=15 * i,
+                       xoffset=(9 * it + 5 * i) % (XMAX[variant] + 1), yoffset=(it + 2 * i) % 8,
+                       border_color=(0x22 + 0x41 * it + 0x9 * i) & 0x1ff)
+        rig.frames_host([h.data_ptr() for h in host])
+        rig.check("%s frames_host field %d" % (variant, it))
         for i in range(n):
-            got = host[i].numpy()
+            got, want = host[i].numpy(), rig.oras[i].out
             rows = np.zeros(outh, dtype=bool)
-            for l in b.get_lines(i):
+            for l in rig.b.get_lines(i):
                 if l.beg >= 0:
                     rows[l.beg:l.beg + max(1, l.end - 1 - l.beg)] = True
             assert rows.any()
-            assert np.array_equal(got[rows], oras[i].out[rows]), (variant, it, i, S.diff_report("rows", got[rows], oras[i].out[rows]))
-            assert np.array_equal(outs[i].cpu().numpy(), oras[i].out), (variant, it, i)
-    b.close()
+            assert np.array_equal(got[rows], want[rows]), (variant, it, i, S.diff_report("rows", got[rows], want[rows]))
+    rig.close()
 
 
 def check_line_blocks(variant, world=2, outw=832, outh=624, fields=5):

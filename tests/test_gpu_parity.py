@@ -12,27 +12,10 @@ import pytest
 
 import support as S
 from ntsc_crt_b200 import layout
+from support import check, run_all, trio
 
 pytestmark = pytest.mark.gpu
-
-
-def trio(variant, outw, outh, fmt=layout.PIX_BGRA):
-    gpu = S.ProductEngine(variant, outw, outh, fmt)
-    ora = S.OracleEngine(variant, outw, outh, fmt)
-    ref = S.RefEngine(variant, outw, outh, fmt, seed=1) if S.have_ref(variant) else None
-    return gpu, ora, ref
-
-
-def run_all(engines, fn):
-    for e in engines:
-        if e is not None:
-            fn(e)
-
-
-def check(gpu, ora, ref, what):
-    S.assert_same_state(gpu.state(), ora.state(), what + " [gpu vs oracle]")
-    if ref is not None:
-        S.assert_same_state(gpu.state(), ref.state(), what + " [gpu vs reference]")
+BGRA = layout.PIX_BGRA
 
 
 @pytest.mark.parametrize("progressive", [True, False])
@@ -224,38 +207,6 @@ def test_dropin_nesrgb(fmt, outw, outh):
         check(gpu, ora, ref, "nesrgb demod %d" % it)
 
 
-def test_batch_snes_matches_oracle():
-    import torch
-    from ntsc_crt_b200 import capi
-    n = 3
-    b = capi.Batch("snes", n)
-    outs, oras, imgs = [], [], []
-    for i in range(n):
-        t = torch.zeros(480, 640, 4, dtype=torch.uint8, device="cuda")
-        outs.append(t)
-        b.set_monitor(i, t, fmt=layout.PIX_BGRA, noise=4 * i, blend=i & 1, scanlines=1, saturation=9 + i)
-        o = S.OracleEngine("snes", 640, 480)
-        o.set(blend=i & 1, scanlines=1, saturation=9 + i)
-        oras.append(o)
-        imgs.append(S.rand_image(256 + 32 * i, 224, seed=200 + i))
-    b.commit_monitors()
-    dimgs = [torch.from_numpy(im).cuda() for im in imgs]
-    for it in range(4):
-        for i in range(n):
-            kw = dict(format=layout.PIX_BGRA, as_color=1, hue=15 * i, dot_crawl_offset=(it + i) % 3)
-            b.set_source(i, dimgs[i], **kw)
-            oras[i].modulate(imgs[i], **kw)
-            oras[i].demodulate(4 * i)
-        b.modulate()
-        b.demodulate()
-        torch.cuda.synchronize()
-        for i in range(n):
-            got = outs[i].cpu().numpy()
-            assert np.array_equal(got, oras[i].out), "snes batch monitor %d field %d: %s" % (
-                i, it, S.diff_report("out", got, oras[i].out))
-    b.close()
-
-
 @pytest.mark.parametrize("variant", ["nes", "nes_p0"])
 def test_dropin_nes(variant):
     """config 3: NES PPU pixels incl. CRT_CHROMA_PATTERN 0, dot crawl cycling 0,1,2."""
@@ -292,40 +243,86 @@ def test_dropin_vhs(color):
         S.assert_same_state(gpu.state(), ora.state(), "vhs demod %d" % it)
 
 
-def test_batch_matches_independent_oracles():
-    """crtx batch of 5 monitors with different knobs / noise = 5 independent reference instances."""
-    import torch
-    from ntsc_crt_b200 import capi
-    n = 5
-    imgs = [S.rand_image(200 + 40 * i, 150 + 30 * i, seed=i) for i in range(n)]
-    b = capi.Batch("ntsc", n)
-    outs = [torch.zeros(480, 640, 4, dtype=torch.uint8, device="cuda") for _ in range(n)]
-    dimg = [torch.from_numpy(x).cuda() for x in imgs]
-    oras = []
-    for i in range(n):
-        knobs = dict(hue=10 * i, saturation=8 + i, contrast=170 + 5 * i, blend=i & 1, scanlines=1)
-        b.set_monitor(i, outs[i], noise=6 * i, **knobs)
-        o = S.OracleEngine("ntsc", 640, 480)
-        o.set(**knobs)
-        oras.append(o)
-    b.commit_monitors()
-    for step in range(3):
-        for i in range(n):
-            b.set_source(i, dimg[i], format=layout.PIX_BGRA, as_color=1, field=step & 1, frame=0)
-        b.modulate()
-        b.demodulate()
-        for i in range(n):
-            oras[i].modulate(imgs[i], format=layout.PIX_BGRA, as_color=1, field=step & 1, frame=0)
-            oras[i].demodulate(6 * i)
-        torch.cuda.synchronize()
-        st = b.get_state()
-        for i in range(n):
-            got = dict(analog=b.signal(i, "analog"), inp=b.signal(i, "inp"), out=outs[i].cpu().numpy(),
-                       ccf=np.array([[st[i].ccf[r][x] for x in range(4)] for r in range(1)]),
-                       hsync=st[i].hsync, vsync=st[i].vsync, rn=st[i].rn)
-            S.assert_same_state(got, oras[i].state(), "batch monitor %d step %d" % (i, step))
-    assert b.launches >= 3 * 5  # modulate 2-3, noise, sync, line kernel per geometry group
-    b.close()
+# The crtx_* batch interface, one case per system: n monitors with their own knobs, noise (and, on VHS, rand() seed) and
+# source image, driven for `fields` fields.  mon(i): monitor i; img(i): its source image; src(it, i): its settings in
+# field it.
+BATCH_CASES = {
+    # 5 independent reference instances
+    "ntsc": dict(n=5, fields=3,
+                 mon=lambda i: dict(noise=6 * i, knobs=dict(hue=10 * i, saturation=8 + i, contrast=170 + 5 * i, blend=i & 1, scanlines=1)),
+                 img=lambda i: S.rand_image(200 + 40 * i, 150 + 30 * i, seed=i),
+                 src=lambda it, i: dict(format=BGRA, as_color=1, field=it & 1, frame=0)),
+    "snes": dict(n=3, fields=4,
+                 mon=lambda i: dict(noise=4 * i, knobs=dict(blend=i & 1, scanlines=1, saturation=9 + i)),
+                 img=lambda i: S.rand_image(256 + 32 * i, 224, seed=200 + i),
+                 src=lambda it, i: dict(format=BGRA, as_color=1, hue=15 * i, dot_crawl_offset=(it + i) % 3)),
+    "template": dict(n=3, fields=4,
+                     mon=lambda i: dict(noise=4 * i, knobs=dict(blend=i & 1, scanlines=1, saturation=9 + i)),
+                     img=lambda i: S.rand_image(256 + 32 * i, 224, seed=300 + i),
+                     src=lambda it, i: dict(format=BGRA, as_color=int(i != 1), hue=15 * i, dot_crawl_offset=(it + i) % 4,
+                                            field=it & 1, frame=(it >> 1) & 1)),
+    # monitor 0 decodes a bright flat picture: wide lines
+    "ntsc_bloom": dict(n=4, fields=4,
+                       mon=lambda i: dict(noise=20 * i, knobs=dict(blend=i & 1, scanlines=1 - (i >> 1), contrast=170 + 10 * i)),
+                       img=lambda i: S.rand_image(256 + 32 * i, 224, seed=400 + i) if i else np.full((200, 300, 4), 250, dtype=np.uint8),
+                       src=lambda it, i: dict(format=BGRA, as_color=1, hue=15 * i, field=it & 1, frame=(it >> 1) & 1)),
+    "ntsc_conv": dict(n=5, fields=4,
+                      mon=lambda i: dict(noise=3 * i, knobs=dict(blend=i & 1, scanlines=(i >> 1) & 1, saturation=8 + i, hue=10 * i)),
+                      img=lambda i: S.rand_image(320 + 16 * i, 240, seed=100 + i),
+                      src=lambda it, i: dict(format=BGRA, as_color=1, field=it & 1, frame=(it >> 1) & 1)),
+    # config 5: noise and aberration draws come from the per-monitor replica of glibc's rand() (crtx_seed), in the
+    # reference's draw order -- against the oracle driven by the same seeds (which tests/test_oracle_vs_ref.py pins
+    # against the real libc stream)
+    "vhs": dict(n=3, fields=4, size=(832, 624),
+                mon=lambda i: dict(noise=24, seed=(1, 42, 2024)[i], knobs=dict(blend=1, scanlines=1)),
+                img=lambda i: S.bars_image(832, 624),
+                src=lambda it, i: dict(format=BGRA, as_color=1 - (i & 1), field=it & 1, frame=(it >> 1) & 1,
+                                       do_aberration=int(it == 2))),
+}
+BATCH_CASES["pv1k"] = BATCH_CASES["template"]  # five samples per chroma period (ccf 5 x 5)
+
+
+@pytest.mark.parametrize("variant", list(BATCH_CASES))
+def test_batch_matches_the_oracle(variant):
+    """a crtx batch equals one oracle per monitor: the whole state of every monitor after every field"""
+    c = BATCH_CASES[variant]
+    outw, outh = c.get("size", (640, 480))
+    rig = S.BatchRig(variant, [dict(outw=outw, outh=outh, fmt=BGRA, **c["mon"](i)) for i in range(c["n"])])
+    imgs = [c["img"](i) for i in range(c["n"])]
+    for it in range(c["fields"]):
+        for i in range(c["n"]):
+            rig.source(i, imgs[i], **c["src"](it, i))
+        rig.modulate()
+        rig.demodulate()
+        rig.check("%s field %d" % (variant, it))
+    if variant == "ntsc":
+        assert rig.b.launches >= 3 * 5  # modulate 2-3, noise, sync, line kernel per geometry group
+    rig.close()
+
+
+def test_batch_rig_names_the_key_that_differs():
+    """BatchRig.check compares every part of the state: a byte of the oracle's out, analog or inp, one ccf entry or hsync
+    changed after a field makes it fail, naming that key"""
+    rig = S.BatchRig("ntsc", [dict(outw=320, outh=240, fmt=BGRA, noise=3, knobs=dict(blend=1, scanlines=1))])
+    rig.source(0, S.rand_image(256, 240, seed=5), format=BGRA, as_color=1, field=0, frame=0)
+    rig.modulate()
+    rig.demodulate()
+    rig.check("field 0")
+    o = rig.oras[0]
+    n = o.spec.input_size
+    pokes = [("out", o.out, (100, 150, 1)), ("analog", np.ctypeslib.as_array(o.mon.analog, shape=(n,)), n // 2),
+             ("inp", np.ctypeslib.as_array(o.mon.inp, shape=(n,)), n // 3), ("ccf", np.ctypeslib.as_array(o.mon.ccf), (0, 2))]
+    for key, arr, at in pokes:
+        arr[at] ^= 1
+        with pytest.raises(AssertionError, match=r"\} %s: " % key):
+            rig.check("%s poked" % key)
+        arr[at] ^= 1
+    o.mon.hsync += 1
+    with pytest.raises(AssertionError, match=r"\} hsync: "):
+        rig.check("hsync poked")
+    o.mon.hsync -= 1
+    rig.check("restored")
+    rig.close()
 
 
 @pytest.mark.parametrize("outw,outh,fmt,blend,scanlines", [
@@ -359,44 +356,3 @@ def test_dropin_ntsc_source_geometries(w, h, fmt):
         check(gpu, ora, ref, "source %dx%d mod %d" % (w, h, it))
         run_all((gpu, ora, ref), lambda e: e.demodulate(0))
         check(gpu, ora, ref, "source %dx%d demod %d" % (w, h, it))
-
-
-def test_batch_vhs_device_rand_replica_matches_glibc_stream():
-    """config 5 in the batch interface: noise and aberration draws come from the per-monitor replica of
-    glibc's rand() (crtx_seed), in the reference's draw order -- compared with the oracle driven by the
-    same seeds (which tests/test_oracle_vs_ref.py pins against the real libc stream)."""
-    import torch
-    from ntsc_crt_b200 import capi
-    n = 3
-    seeds = [1, 42, 2024]
-    img = S.bars_image(832, 624)
-    dimg = torch.from_numpy(img).cuda()
-    b = capi.Batch("vhs", n)
-    outs = [torch.zeros(624, 832, 4, dtype=torch.uint8, device="cuda") for _ in range(n)]
-    oras = []
-    for i in range(n):
-        b.set_monitor(i, outs[i], noise=24, blend=1, scanlines=1)
-        b.seed(seeds[i], first=i, count=1)
-        o = S.OracleEngine("vhs", 832, 624, seed=seeds[i])
-        o.set(blend=1, scanlines=1)
-        oras.append(o)
-    b.commit_monitors()
-    for step in range(4):
-        aberr = 1 if step == 2 else 0
-        for i in range(n):
-            b.set_source(i, dimg, format=layout.PIX_BGRA, as_color=1 - (i & 1), field=step & 1, frame=(step >> 1) & 1,
-                         do_aberration=aberr)
-            oras[i].modulate(img, format=layout.PIX_BGRA, as_color=1 - (i & 1), field=step & 1, frame=(step >> 1) & 1,
-                             do_aberration=aberr)
-        b.modulate()
-        b.demodulate()
-        for i in range(n):
-            oras[i].demodulate(24)
-        torch.cuda.synchronize()
-        st = b.get_state()
-        for i in range(n):
-            got = dict(analog=b.signal(i, "analog"), inp=b.signal(i, "inp"), out=outs[i].cpu().numpy(),
-                       ccf=np.array([[st[i].ccf[0][x] for x in range(4)]]),
-                       hsync=st[i].hsync, vsync=st[i].vsync, rn=st[i].rn)
-            S.assert_same_state(got, oras[i].state(), "vhs batch monitor %d step %d" % (i, step))
-    b.close()

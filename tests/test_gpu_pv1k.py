@@ -1,12 +1,11 @@
 """SURVEY 8f-3: CRT_SYSTEM_PV1K (crt_pv1k.c:120-331 and the CRT_CC_SAMPLES == 5 branches of crt_core.c:282, 459-467,
 480-509, 545-549): 1920 samples per line, FIVE samples per chroma period, a 5-line chroma cycle, vertical sync at the
 bottom of the field -- through libcrt_b200_pv1k.so, bit for bit against the oracle and the compiled reference."""
-import numpy as np
 import pytest
 
 import support as S
 from ntsc_crt_b200 import layout
-from test_gpu_parity import check, run_all, trio
+from support import check, run_all, trio
 
 pytestmark = pytest.mark.gpu
 
@@ -39,44 +38,6 @@ def test_dropin_pv1k_source_geometries(w, h):
                                                       hue=33 * it, dot_crawl_offset=it, yoffset=it & 1))
         run_all((gpu, ora, ref), lambda e: e.demodulate(5 * it))
         check(gpu, ora, ref, "pv1k %dx%d call %d" % (w, h, it))
-
-
-def test_batch_pv1k_matches_oracle():
-    import torch
-    from ntsc_crt_b200 import capi
-    n = 3
-    b = capi.Batch("pv1k", n)
-    outs, oras, imgs = [], [], []
-    for i in range(n):
-        t = torch.zeros(480, 640, 4, dtype=torch.uint8, device="cuda")
-        outs.append(t)
-        b.set_monitor(i, t, fmt=layout.PIX_BGRA, noise=4 * i, blend=i & 1, scanlines=1, saturation=9 + i)
-        o = S.OracleEngine("pv1k", 640, 480)
-        o.set(blend=i & 1, scanlines=1, saturation=9 + i)
-        oras.append(o)
-        imgs.append(S.rand_image(256 + 32 * i, 224, seed=300 + i))
-    b.commit_monitors()
-    dimgs = [torch.from_numpy(im).cuda() for im in imgs]
-    for it in range(4):
-        for i in range(n):
-            kw = dict(format=layout.PIX_BGRA, as_color=1 if i != 1 else 0, hue=15 * i, dot_crawl_offset=(it + i) % 4,
-                      field=it & 1, frame=(it >> 1) & 1)
-            b.set_source(i, dimgs[i], **kw)
-            oras[i].modulate(imgs[i], **kw)
-            oras[i].demodulate(4 * i)
-        b.modulate()
-        b.demodulate()
-        torch.cuda.synchronize()
-        st = b.get_state()
-        for i in range(n):
-            got = outs[i].cpu().numpy()
-            assert np.array_equal(got, oras[i].out), "pv1k batch monitor %d field %d: %s" % (
-                i, it, S.diff_report("out", got, oras[i].out))
-            assert np.array_equal(b.signal(i, "analog"), oras[i].analog), (i, it)
-            assert np.array_equal(b.signal(i, "inp"), oras[i].inp), (i, it)
-            assert [[st[i].ccf[r][x] for x in range(5)] for r in range(5)] == oras[i].ccf.tolist(), (i, it)
-            assert (st[i].hsync, st[i].vsync, st[i].rn) == (oras[i].hsync, oras[i].vsync, oras[i].rn), (i, it)
-    b.close()
 
 
 def test_dropin_pv1k_generic_equaliser_and_geometries():

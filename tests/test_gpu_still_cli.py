@@ -2,7 +2,6 @@
 it writes must be byte-identical to what the all-reference build of crt_main.c (oracle/_ref/cli_ref_ntsc) writes for
 that pair alone -- PPM and BMP, in and out, every flag of the command line, several images in one run."""
 import os
-import struct
 import subprocess
 
 import numpy as np
@@ -16,22 +15,6 @@ REF_CLI = os.path.join(S.REF_DIR, "cli_ref_ntsc")
 STILL = os.path.join(S.ROOT, "ntsc-crt_b200", "bin", "crtx_still")
 
 
-def write_ppm(path, rgb, maxc=255, comment=False):
-    with open(path, "wb") as f:
-        f.write(b"P6\n" + (b"# made by a test\n" if comment else b"") + b"%d %d\n%d\n" % (rgb.shape[1], rgb.shape[0], maxc))
-        f.write(rgb.tobytes())
-
-
-def write_bmp(path, bgra, bits):
-    h, w = bgra.shape[:2]
-    bpp = bits // 8
-    pad = (4 - (w * bpp) % 4) % 4
-    rows = b"".join(bgra[y, :, :bpp].tobytes() + b"\0" * pad for y in range(h - 1, -1, -1))
-    head = b"BM" + struct.pack("<IHHI", 54 + len(rows), 0, 0, 54) + struct.pack("<IiiHHIIiiII", 40, w, h, 1, bits, 0, len(rows), 0, 0, 0, 0)
-    with open(path, "wb") as f:
-        f.write(head + rows)
-
-
 @pytest.mark.skipif(not (os.path.exists(REF_CLI) and os.path.exists(STILL)), reason="driver binaries not built")
 @pytest.mark.parametrize("flags,outw,outh,noise,hue", [("-o", 832, 624, 0, 0), ("-op", 640, 480, 12, 30), ("-omf", 333, 250, 24, 0),
                                                        ("-opr", 832, 624, 0, 90), ("-opa", 320, 240, 0, 0)])
@@ -39,19 +22,19 @@ def test_batch_still_driver_is_byte_identical_to_the_reference_cli(tmp_path, fla
     rng = np.random.default_rng(outw + noise)
     inputs = []
     a = S.bars_image(320, 240, fmt=S.layout.PIX_RGB)[..., :3].copy()
-    write_ppm(str(tmp_path / "a.ppm"), a)
+    S.write_ppm(str(tmp_path / "a.ppm"), a)
     inputs.append(("a.ppm", "a_out.ppm"))
     b = rng.integers(0, 256, size=(200, 301, 3), dtype=np.uint8)  # odd width, comment line in the header
-    write_ppm(str(tmp_path / "b.ppm"), b, comment=True)
+    S.write_ppm(str(tmp_path / "b.ppm"), b, comment=True)
     inputs.append(("b.ppm", "b_out.bmp"))
     c = rng.integers(0, 101, size=(64, 48, 3), dtype=np.uint8)  # maximum colour value 100: rescaled (ppm_rw.c:80)
-    write_ppm(str(tmp_path / "c.ppm"), c, maxc=100)
+    S.write_ppm(str(tmp_path / "c.ppm"), c, maxc=100)
     inputs.append(("c.ppm", "c_out.ppm"))
     d = S.rand_image(257, 199, seed=4)
-    write_bmp(str(tmp_path / "d.bmp"), d, 24)
+    S.write_bmp(str(tmp_path / "d.bmp"), d, 24)
     inputs.append(("d.bmp", "d_out.bmp"))
     e = S.rand_image(640, 480, seed=5)
-    write_bmp(str(tmp_path / "e.bmp"), e, 32)
+    S.write_bmp(str(tmp_path / "e.bmp"), e, 32)
     inputs.append(("e.bmp", "e_out.ppm"))
     args = []
     for i, o in inputs:

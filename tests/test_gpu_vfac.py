@@ -13,7 +13,7 @@ import support as S
 import test_oracle_vfac as V
 from ntsc_crt_b200 import layout
 from test_gpu_lineshard import decode_one_image_in_blocks
-from test_gpu_parity import check, run_all, trio
+from support import check, run_all, trio
 
 pytestmark = pytest.mark.gpu
 

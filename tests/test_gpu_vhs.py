@@ -114,83 +114,6 @@ def test_dropin_random_cases(seed):
 # the batch interface
 # ----------------------------------------------------------------------------------
 
-def seed_oracle(ora, seed):
-    ora.lib.ocrt_rand_seed(C.byref(ora.rand), seed)
-
-
-class Rig:
-    """a VHS batch and one oracle per monitor, driven through the same calls; mons[i] = dict(seed, noise, fmt, outw,
-    outh, knobs)"""
-
-    def __init__(self, mons):
-        import torch
-        from ntsc_crt_b200 import capi
-        self.mons = mons
-        self.b = capi.Batch("vhs", len(mons))
-        self.outs, self.oras, self._dev = [], [], {}
-        for i, m in enumerate(mons):
-            out = torch.zeros(m["outh"], m["outw"], max(1, layout.bpp4fmt(m["fmt"])), dtype=torch.uint8, device="cuda")
-            self.b.set_monitor(i, out, fmt=m["fmt"], noise=m["noise"], **m["knobs"])
-            self.b.seed(m["seed"], first=i, count=1)
-            o = S.OracleEngine("vhs", m["outw"], m["outh"], m["fmt"], seed=m["seed"])
-            o.set(**m["knobs"])
-            self.outs.append(out)
-            self.oras.append(o)
-        self.b.commit_monitors()
-
-    def device(self, img):
-        import torch
-        if id(img) not in self._dev:
-            self._dev[id(img)] = (img, torch.from_numpy(img).cuda())
-        return self._dev[id(img)][1]
-
-    def seed(self, seed, first, count):
-        self.b.seed(seed, first=first, count=count)
-        for i in range(first, first + count):
-            seed_oracle(self.oras[i], seed)
-            self.mons[i]["seed"] = seed
-
-    def modulate(self, calls, first=0, count=None):
-        """calls[i] = (image, settings) for the monitors i of [first, first + count)"""
-        count = len(self.mons) - first if count is None else count
-        for i in range(first, first + count):
-            img, kw = calls[i]
-            self.b.set_source(i, self.device(img), **kw)
-            self.oras[i].modulate(img, **kw)
-        self.b.modulate(first=first, count=count)
-
-    def demodulate(self, first=0, count=None):
-        count = len(self.mons) - first if count is None else count
-        self.b.demodulate(first=first, count=count)
-        for i in range(first, first + count):
-            self.oras[i].demodulate(self.mons[i]["noise"])
-
-    def frames_host(self, calls, host):
-        """crtx_frames_host: modulate from host images, demodulate, copy the images to host[i]"""
-        for i, (img, kw) in enumerate(calls):
-            s = self.b.sources[i]
-            s.data, s.h, s.w, s.pitch = img.ctypes.data, img.shape[0], img.shape[1], 0
-            for k, v in kw.items():
-                setattr(s, k, v)
-            self.oras[i].modulate(img, **kw)
-            self.oras[i].demodulate(self.mons[i]["noise"])
-        self.b.frames_host([h.ctypes.data for h in host])
-
-    def check(self, what):
-        import torch
-        torch.cuda.synchronize()
-        st = self.b.get_state()
-        for i, o in enumerate(self.oras):
-            got = dict(analog=self.b.signal(i, "analog"), inp=self.b.signal(i, "inp"), out=self.outs[i].cpu().numpy(),
-                       ccf=np.array([[st[i].ccf[r][x] for x in range(SPEC.cc_samples)] for r in range(SPEC.vper)]),
-                       hsync=st[i].hsync, vsync=st[i].vsync, rn=st[i].rn)
-            m = self.mons[i]
-            S.assert_same_state(got, o.state(), "%s, monitor %d (seed %d, noise %d, out fmt %d)" % (what, i, m["seed"], m["noise"], m["fmt"]))
-
-    def close(self):
-        self.b.close()
-
-
 def field_settings(rng, it, src_fmt=layout.PIX_BGRA, aberration=0):
     return dict(format=src_fmt, as_color=int(rng.integers(0, 2)), field=it & 1, frame=(it >> 1) & 1, raw=0,
                 hue=int(rng.integers(0, 360)), xoffset=int(rng.integers(0, 16)), yoffset=int(rng.integers(0, 3)),
@@ -222,14 +145,13 @@ def test_batch_many_generator_states():
         knobs = dict(blend=0 if aberr else i & 1, scanlines=(i >> 1) & 1, hue=int(rng.integers(-60, 60)),
                      saturation=int(rng.integers(5, 30)))
         mons.append(dict(seed=seeds[i], noise=noise, fmt=fmt, outw=outw, outh=outh, knobs=knobs, aberr=aberr))
-    rig = Rig(mons)
+    rig = S.BatchRig("vhs", mons)
     imgs = sources(rng)
     for it in range(FIELDS):
-        calls = {}
         for i, m in enumerate(mons):
             img, fmt = imgs[(i + it) % len(imgs)]
-            calls[i] = (img, field_settings(rng, it, fmt, int(m["aberr"])))
-        rig.modulate(calls)
+            rig.source(i, img, **field_settings(rng, it, fmt, int(m["aberr"])))
+        rig.modulate()
         rig.check("field %d modulate" % it)
         rig.demodulate()
         rig.check("field %d demodulate" % it)
@@ -243,7 +165,7 @@ def test_batch_subranges_and_reseeding():
     n = 6
     mons = [dict(seed=SEEDS[i], noise=(24, 3, 255, 12, 40, 1 << 20)[i], fmt=layout.PIX_BGRA, outw=320, outh=240,
                  knobs=dict(blend=0, scanlines=i & 1)) for i in range(n)]
-    rig = Rig(mons)
+    rig = S.BatchRig("vhs", mons)
     imgs = sources(rng, 2)
     # (first, count) of each step; None: re-seed monitors 2 and 3 with a fresh seed before the step
     steps = [(0, n), (1, 3), (0, 1), (n - 2, 2), None, (2, 3), (0, n), (5, 1), (0, n)]
@@ -253,8 +175,10 @@ def test_batch_subranges_and_reseeding():
             rig.seed(0xDEADBEEF, first=2, count=2)
             continue
         first, count = step
-        calls = {i: (imgs[(i + it) % 2][0], field_settings(rng, it, imgs[(i + it) % 2][1], int(i == 3))) for i in range(first, first + count)}
-        rig.modulate(calls, first, count)
+        for i in range(first, first + count):
+            img, fmt = imgs[(i + it) % 2]
+            rig.source(i, img, **field_settings(rng, it, fmt, int(i == 3)))
+        rig.modulate(first, count)
         rig.check("step %d [%d, %d) modulate" % (it, first, first + count))
         rig.demodulate(first, count)
         rig.check("step %d [%d, %d) demodulate" % (it, first, first + count))
@@ -273,15 +197,14 @@ def test_batch_unknown_formats():
     fmts = [layout.PIX_BGRA, layout.PIX_RGB, 9, layout.PIX_BGRA, layout.PIX_ARGB, layout.PIX_BGRA]
     mons = [dict(seed=SEEDS[(i + 1) % len(SEEDS)], noise=(24, 12, 24, 40, 3, 255)[i], fmt=fmts[i], outw=320, outh=240,
                  knobs=dict(blend=0, scanlines=1)) for i in range(n)]
-    rig = Rig(mons)
+    rig = S.BatchRig("vhs", mons)
     imgs = sources(rng, 2)
     for it in range(6):
-        calls = {}
         for i in range(n):
             img, fmt = imgs[(i + it) % 2]
             unknown, aberr = {0: (it & 1, 1), 1: (it & 1, 0), 2: (0, 1), 3: (0, 1), 4: (it % 3 == 1, 1), 5: (0, 0)}[i]
-            calls[i] = (img, field_settings(rng, it, int(rng.choice(UNKNOWN_FORMATS)) if unknown else fmt, aberr))
-        rig.modulate(calls)
+            rig.source(i, img, **field_settings(rng, it, int(rng.choice(UNKNOWN_FORMATS)) if unknown else fmt, aberr))
+        rig.modulate()
         rig.check("field %d modulate" % it)
         rig.demodulate()
         rig.check("field %d demodulate" % it)
@@ -295,15 +218,14 @@ def test_frames_host_with_aberration():
     n = 3
     mons = [dict(seed=SEEDS[i + 2], noise=(24, 12, 40)[i], fmt=layout.PIX_BGRA, outw=400, outh=300,
                  knobs=dict(blend=0, scanlines=1)) for i in range(n)]
-    rig = Rig(mons)
+    rig = S.BatchRig("vhs", mons)
     imgs = sources(rng, n)
     host = [np.full((300, 400, 4), 0xA5, dtype=np.uint8) for _ in range(n)]
     for it in range(4):
-        calls = []
         for i in range(n):
             img, fmt = imgs[i]
-            calls.append((img, field_settings(rng, it, 9 if (i == 1 and it % 2 == 0) else fmt, int(i != 2))))
-        rig.frames_host(calls, host)
+            rig.source(i, img, **field_settings(rng, it, 9 if (i == 1 and it % 2 == 0) else fmt, int(i != 2)))
+        rig.frames_host([h.ctypes.data for h in host])
         rig.check("frames_host field %d" % it)
         for i in range(n):
             assert np.array_equal(host[i], rig.oras[i].out), "field %d monitor %d: %s" % (it, i, S.diff_report("host image", host[i], rig.oras[i].out))
@@ -318,7 +240,7 @@ def test_dropin_and_batch_draw_the_same_stream():
     noises = [24, -40, 1 << 23]
     mons = [dict(seed=s, noise=noises[i], fmt=layout.PIX_BGRA, outw=400, outh=300, knobs=dict(blend=0, scanlines=1))
             for i, s in enumerate(seeds)]
-    rig = Rig(mons)
+    rig = S.BatchRig("vhs", mons)
     imgs = sources(rng, 2)
     fields = []
     for it in range(5):
@@ -326,14 +248,13 @@ def test_dropin_and_batch_draw_the_same_stream():
                        for i in range(len(seeds))})
     states = {}
     for it, calls in enumerate(fields):
-        rig.modulate(calls)
+        for i, (img, kw) in calls.items():
+            rig.source(i, img, **kw)
+        rig.modulate()
         rig.demodulate()
         rig.check("field %d" % it)
-        st = rig.b.get_state()
         for i in range(len(seeds)):
-            states[(i, it)] = dict(analog=rig.b.signal(i, "analog"), inp=rig.b.signal(i, "inp"), out=rig.outs[i].cpu().numpy().copy(),
-                                   ccf=np.array([[st[i].ccf[r][x] for x in range(SPEC.cc_samples)] for r in range(SPEC.vper)]),
-                                   hsync=st[i].hsync, vsync=st[i].vsync, rn=st[i].rn)
+            states[(i, it)] = S.monitor_state(rig.b, i, rig.outs[i])
     rig.close()
     for i, s in enumerate(seeds):
         gpu = S.ProductEngine("vhs", 400, 300)

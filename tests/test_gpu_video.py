@@ -9,23 +9,12 @@ from ntsc_crt_b200 import layout
 pytestmark = pytest.mark.gpu
 
 
-def moving_bars(n, w, h, seed=0):
-    rng = np.random.default_rng(seed)
-    base = S.bars_image(w, h)
-    frames = []
-    for k in range(n):
-        f = np.roll(base, 7 * k, axis=1).copy()
-        f[..., :3] ^= rng.integers(0, 16, size=(h, w, 3), dtype=np.uint8)  # every frame differs
-        frames.append(f)
-    return np.stack(frames)
-
-
 @pytest.mark.parametrize("noise,segments", [(0, 5), (12, 4)])
 def test_video_sequence_matches_sequential_reference_loop(noise, segments):
     import torch
     from ntsc_crt_b200 import video
     n, w, h = 23, 320, 240
-    frames = moving_bars(n, w, h)
+    frames = S.moving_bars(n, w, h)
     ora = S.OracleEngine("ntsc", 640, 480)
     ora.set(blend=0, scanlines=1, saturation=10)
     want = []

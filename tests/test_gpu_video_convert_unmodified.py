@@ -6,14 +6,10 @@ output/ files must be byte-identical; the reference build is also pinned to the 
 the cleared stack really gave xoffset = yoffset = 0."""
 import os
 import shutil
-import subprocess
 
-import numpy as np
 import pytest
 
 import support as S
-from ntsc_crt_b200 import layout
-from test_gpu_video_driver import moving_bars, read_bmp32, write_bmp24, write_bmp32
 
 REF_VIDEO = os.path.join(S.REF_DIR, "video_ref_ntsc_z")
 B200_VIDEO = os.path.join(S.REF_DIR, "video_b200_ntsc_z")
@@ -21,25 +17,14 @@ B200_VIDEO = os.path.join(S.REF_DIR, "video_b200_ntsc_z")
 pytestmark = pytest.mark.gpu
 
 
-def run_driver(exe, where, frames, flags, outw, outh, noise, bits=24):
-    os.makedirs(os.path.join(where, "frames"))
-    os.makedirs(os.path.join(where, "output"))
-    for k in range(len(frames)):
-        (write_bmp24 if bits == 24 else write_bmp32)(os.path.join(where, "frames", "%06d.bmp" % (k + 1)), frames[k])
-    # video_convert.c:244: `while (err < nframes)` from 1 -- num_frames - 1 images are converted
-    subprocess.run([exe, flags, str(len(frames) + 1), str(outw), str(outh), str(noise)], cwd=where, check=True,
-                   stdout=subprocess.DEVNULL, timeout=600)
-    return [open(os.path.join(where, "output", "%06d.bmp" % (k + 1)), "rb").read() for k in range(len(frames))]
-
-
 @pytest.mark.skipif(not (os.path.exists(REF_VIDEO) and os.path.exists(B200_VIDEO)), reason="oracle/_ref video drivers not built")
 @pytest.mark.parametrize("flags,noise,w,bits", [("-o", 0, 320, 24), ("-o", 12, 333, 24), ("-om", 3, 320, 32), ("-osp", 0, 256, 24)])
 def test_unmodified_video_convert_runs_against_the_library(tmp_path, flags, noise, w, bits):
     """the same unmodified driver source linked against libcrt_b200_ntsc.so writes byte-identical files (12 images,
     interlaced / progressive, colour / monochrome, scanline gaps filled or not, noise, odd widths, 24- and 32-bit input)"""
-    frames = moving_bars(12, w, 240, seed=5)
-    ref = run_driver(REF_VIDEO, str(tmp_path / "ref"), frames, flags, 640, 480, noise, bits)
-    got = run_driver(B200_VIDEO, str(tmp_path / "b200"), frames, flags, 640, 480, noise, bits)
+    frames = S.moving_bars(12, w, 240, seed=5)
+    ref = S.run_video_convert(REF_VIDEO, str(tmp_path / "ref"), frames, flags, 640, 480, noise, bits)
+    got = S.run_video_convert(B200_VIDEO, str(tmp_path / "b200"), frames, flags, 640, 480, noise, bits)
     for k, (a, b) in enumerate(zip(got, ref)):
         assert a == b, "output/%06d.bmp differs from the reference build's" % (k + 1)
     shutil.rmtree(str(tmp_path / "ref"))

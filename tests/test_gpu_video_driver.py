@@ -2,7 +2,6 @@
 sequential loop of extra/video_convert.c:226-277 run on the oracle: same BMP files in, same pixels (and the
 same BMP container bmp_rw.c:96-146 writes) out."""
 import os
-import struct
 import subprocess
 
 import numpy as np
@@ -16,55 +15,16 @@ pytestmark = pytest.mark.gpu
 DRIVER = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "ntsc-crt_b200", "bin", "crtx_video")
 
 
-def write_bmp24(path, bgra):
-    """24-bit bottom-up BMP with row padding, as ffmpeg would hand it to the reference's reader."""
-    h, w = bgra.shape[:2]
-    pad = (4 - (w * 3) % 4) % 4
-    rows = b"".join(bgra[y, :, :3].tobytes() + b"\0" * pad for y in range(h - 1, -1, -1))
-    head = b"BM" + struct.pack("<IHHI", 54 + len(rows), 0, 0, 54) + struct.pack("<IiiHHIIiiII", 40, w, h, 1, 24, 0, len(rows), 0, 0, 0, 0)
-    with open(path, "wb") as f:
-        f.write(head + rows)
-
-
-def write_bmp32(path, bgra):
-    h, w = bgra.shape[:2]
-    rows = b"".join(bgra[y].tobytes() for y in range(h - 1, -1, -1))
-    head = b"BM" + struct.pack("<IHHI", 54 + len(rows), 0, 0, 54) + struct.pack("<IiiHHIIiiII", 40, w, h, 1, 32, 0, len(rows), 0, 0, 0, 0)
-    with open(path, "wb") as f:
-        f.write(head + rows)
-
-
-def read_bmp32(path):
-    raw = open(path, "rb").read()
-    w, h = struct.unpack_from("<ii", raw, 18)
-    bpp = struct.unpack_from("<H", raw, 28)[0]
-    assert raw[:2] == b"BM" and bpp == 32 and struct.unpack_from("<I", raw, 10)[0] == 54
-    assert len(raw) == 54 + w * h * 4 and struct.unpack_from("<I", raw, 2)[0] == len(raw)
-    return np.frombuffer(raw, dtype=np.uint8, offset=54).reshape(h, w, 4)[::-1]
-
-
-def moving_bars(n, w, h, seed=0):
-    rng = np.random.default_rng(seed)
-    base = S.bars_image(w, h)
-    frames = []
-    for k in range(n):
-        f = np.roll(base, 7 * k, axis=1).copy()
-        f[..., :3] ^= rng.integers(0, 16, size=(h, w, 3), dtype=np.uint8)
-        f[..., 3] = 255  # what the reader makes of 24-bit files (bmp_rw.c:90)
-        frames.append(f)
-    return np.stack(frames)
-
-
 @pytest.mark.skipif(not os.path.exists(DRIVER), reason="tools/crtx_video not built")
 @pytest.mark.parametrize("flags,noise,segments,w,bits", [([], 0, 5, 320, 24), ([], 12, 4, 321, 24), (["-m", "-a"], 5, 23, 320, 24),
                                                          (["-p"], 0, 3, 320, 24), ([], 3, 6, 323, 32)])
 def test_batch_video_driver_writes_the_sequential_loops_images(tmp_path, flags, noise, segments, w, bits):
     n, h = 23, 240
-    frames = moving_bars(n, w, h)
+    frames = S.moving_bars(n, w, h)
     os.mkdir(tmp_path / "frames")
     os.mkdir(tmp_path / "output")
     for k in range(n):
-        (write_bmp24 if bits == 24 else write_bmp32)(str(tmp_path / "frames" / ("%06d.bmp" % (k + 1))), frames[k])
+        S.write_bmp(str(tmp_path / "frames" / ("%06d.bmp" % (k + 1))), frames[k], bits)
     res = subprocess.run([DRIVER] + flags + ["-S", str(segments), str(n + 1), "640", "480", str(noise)],
                          cwd=str(tmp_path), stdout=subprocess.PIPE, stderr=subprocess.PIPE, timeout=300)
     assert res.returncode == 0, res.stderr.decode()
@@ -75,7 +35,7 @@ def test_batch_video_driver_writes_the_sequential_loops_images(tmp_path, flags, 
         field, frame = (0, 0) if progressive else (k & 1, (k >> 1) & 1)
         ora.modulate(frames[k], format=layout.PIX_BGRA, as_color=0 if "-m" in flags else 1, field=field, frame=frame)
         ora.demodulate(noise)
-        got = read_bmp32(str(tmp_path / "output" / ("%06d.bmp" % (k + 1))))
+        got = S.read_bmp32(str(tmp_path / "output" / ("%06d.bmp" % (k + 1))))
         assert np.array_equal(got, ora.out), "image %d: %s\n%s" % (k + 1, S.diff_report("image", got, ora.out),
                                                                    res.stdout.decode()[-300:])
     if noise == 0:

@@ -12,8 +12,7 @@ import os
 import pytest
 
 import support as S
-from nes_border_oracle import oracle_engine
-from test_gpu_nes_border import BORDER_VARIANTS, COLOURS, XMAX
+from nes_border_oracle import BORDER_VARIANTS, COLOURS, XMAX, oracle_engine
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "nes_border_ref.json")
 RECORD = os.environ.get("NES_BORDER_RECORD") == "1"

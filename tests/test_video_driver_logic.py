@@ -4,7 +4,6 @@ verification of every seam, repair of a failed segment, BMP reading and writing)
 including the repair path that well-behaved inputs never reach.  The GPU suite runs the same program against
 the real library (tests/test_gpu_video_driver.py)."""
 import os
-import struct
 import subprocess
 
 import numpy as np
@@ -14,22 +13,6 @@ import support as S
 from ntsc_crt_b200 import layout
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def write_bmp24(path, bgra):
-    h, w = bgra.shape[:2]
-    pad = (4 - (w * 3) % 4) % 4
-    rows = b"".join(bgra[y, :, :3].tobytes() + b"\0" * pad for y in range(h - 1, -1, -1))
-    head = b"BM" + struct.pack("<IHHI", 54 + len(rows), 0, 0, 54) + struct.pack("<IiiHHIIiiII", 40, w, h, 1, 24, 0, len(rows), 0, 0, 0, 0)
-    with open(path, "wb") as f:
-        f.write(head + rows)
-
-
-def read_bmp32(path):
-    raw = open(path, "rb").read()
-    w, h = struct.unpack_from("<ii", raw, 18)
-    assert raw[:2] == b"BM" and struct.unpack_from("<H", raw, 28)[0] == 32 and len(raw) == 54 + w * h * 4
-    return np.frombuffer(raw, dtype=np.uint8, offset=54).reshape(h, w, 4)[::-1]
 
 
 @pytest.fixture(scope="module")
@@ -71,7 +54,7 @@ def test_driver_logic_against_the_sequential_loop(tmp_path, driver, flags, noise
     os.mkdir(tmp_path / "frames")
     os.mkdir(tmp_path / "output")
     for k in range(n):
-        write_bmp24(str(tmp_path / "frames" / ("%06d.bmp" % (k + 1))), frames[k])
+        S.write_bmp(str(tmp_path / "frames" / ("%06d.bmp" % (k + 1))), frames[k], 24)
     res = subprocess.run([driver] + flags + ["-S", str(segments), str(n + 1), str(outw), str(outh), str(noise)],
                          cwd=str(tmp_path), stdout=subprocess.PIPE, stderr=subprocess.PIPE, timeout=600)
     assert res.returncode == 0, res.stderr.decode()
@@ -81,7 +64,7 @@ def test_driver_logic_against_the_sequential_loop(tmp_path, driver, flags, noise
         field, frame = (0, 0) if "-p" in flags else (k & 1, (k >> 1) & 1)
         ora.modulate(frames[k], format=layout.PIX_BGRA, as_color=0 if "-m" in flags else 1, field=field, frame=frame)
         ora.demodulate(noise)
-        got = read_bmp32(str(tmp_path / "output" / ("%06d.bmp" % (k + 1))))
+        got = S.read_bmp32(str(tmp_path / "output" / ("%06d.bmp" % (k + 1))))
         assert np.array_equal(got, ora.out), "image %d: %s\n%s" % (k + 1, S.diff_report("image", got, ora.out),
                                                                    res.stdout.decode()[-200:])
     tail = res.stdout.decode().strip().splitlines()[-1]
