@@ -26,6 +26,8 @@
  *      CRT_SYSTEM 4                          libcrt_b200_template.so
  *      CRT_SYSTEM 2                          libcrt_b200_pv1k.so
  *      CRT_SYSTEM 0, CRT_DO_BLOOM 1          libcrt_b200_ntsc_bloom.so
+ *      CRT_SYSTEM 0, CRT_DO_VSYNC 0 / CRT_DO_HSYNC 0 / both 0   libcrt_b200_ntsc_novsync.so / _nohsync.so / _nosync.so
+ *      CRT_SYSTEM 5 / 1, CRT_DO_VSYNC 0, CRT_DO_HSYNC 0        libcrt_b200_vhs_nosync.so / libcrt_b200_nes_nosync.so
  * (and libcrt_b200_ntsc_conv{,6,5,4}.so for the USE_CONVOLUTION builds of crt_core.c:85-88)
  */
 #ifndef CRT_B200_H
@@ -351,8 +353,16 @@ struct NTSC_SETTINGS {
 #ifndef CRT_DO_BLOOM
 #define CRT_DO_BLOOM 0
 #endif
+/* crt_core.h:71-72 (unguarded #defines there, both on): the decoder's sync searches.  With CRT_DO_VSYNC 0 the field is
+ * read from analog[] before the noise is added and the lines are decoded from vsync -3 (crt_core.c:323-342); with
+ * CRT_DO_HSYNC 0 hsync is 0 after every decoded line (crt_core.c:446-450).  Compile the caller with -DCRT_DO_VSYNC=0
+ * and / or -DCRT_DO_HSYNC=0 and link the library built the same way (crtx_do_vsync(), crtx_do_hsync()). */
+#ifndef CRT_DO_VSYNC
 #define CRT_DO_VSYNC 1
+#endif
+#ifndef CRT_DO_HSYNC
 #define CRT_DO_HSYNC 1
+#endif
 
 struct CRT {
     signed char analog[CRT_INPUT_SIZE]; /* encoder output (host mirror, kept coherent) */

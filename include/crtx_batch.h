@@ -89,6 +89,8 @@ typedef struct crtx_line {
 int crtx_system(void);          /* CRT_SYSTEM */
 int crtx_chroma_pattern(void);  /* CRT_CHROMA_PATTERN */
 int crtx_nes_border(void);      /* NES_BORDER: 1 if the NES encoder draws the border colour (crt_nes.c:64-69) */
+int crtx_do_vsync(void);        /* CRT_DO_VSYNC: 0 if the decoder takes the field before the noise, vsync -3 */
+int crtx_do_hsync(void);        /* CRT_DO_HSYNC: 0 if hsync is 0 after every decoded line */
 int crtx_hres(void);            /* CRT_HRES */
 int crtx_input_size(void);      /* CRT_INPUT_SIZE */
 int crtx_lines(void);           /* CRT_LINES */

@@ -19,7 +19,11 @@ VARIANTS = ("ntsc", "ntsc_conv", "ntsc_conv6", "ntsc_conv5", "ntsc_conv4", "vhs"
 # picture.  Kept apart from VARIANTS, whose members all encode what the stock build of their system encodes: code that
 # sweeps VARIANTS against a CPU model of the stock encoders would see a border it does not expect.
 BORDER_VARIANTS = ("nes_border", "nes_p0_border")
-ALL_VARIANTS = VARIANTS + BORDER_VARIANTS
+# Builds with the reference's sync searches off (CRT_DO_VSYNC 0 / CRT_DO_HSYNC 0, crt_core.h:71-72): the field is taken
+# before the noise and the lines decoded from vsync -3, and / or hsync is 0 after every decoded line.  Kept apart from
+# VARIANTS for the same reason: they decode what the stock build of their system does not.
+SYNC_VARIANTS = ("ntsc_novsync", "ntsc_nohsync", "ntsc_nosync", "vhs_nosync", "nes_nosync")
+ALL_VARIANTS = VARIANTS + BORDER_VARIANTS + SYNC_VARIANTS
 
 
 def lib_path(variant):
@@ -77,7 +81,7 @@ class Line(C.Structure):  # crtx_line
 
 CRT_EXPORTS = ("crt_init", "crt_resize", "crt_reset", "crt_modulate", "crt_demodulate",
                "crt_bpp4fmt", "crt_sincos14")
-CRTX_EXPORTS = ("crtx_system", "crtx_chroma_pattern", "crtx_nes_border", "crtx_hres", "crtx_input_size", "crtx_lines",
+CRTX_EXPORTS = ("crtx_system", "crtx_chroma_pattern", "crtx_nes_border", "crtx_do_vsync", "crtx_do_hsync", "crtx_hres", "crtx_input_size", "crtx_lines",
                 "crtx_cc_vper", "crtx_create", "crtx_destroy", "crtx_set_monitors", "crtx_set_state",
                 "crtx_get_state", "crtx_seed", "crtx_analog", "crtx_inp", "crtx_read_signal",
                 "crtx_write_signal", "crtx_modulate",
@@ -125,8 +129,11 @@ def load(variant):
     lib.crtx_get_timing.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_long)]
     lib.crtx_last_error.restype = C.c_char_p
     lib.crtx_nes_border.restype = ip
+    lib.crtx_do_vsync.restype = ip
+    lib.crtx_do_hsync.restype = ip
     assert (lib.crtx_system() == spec.system and lib.crtx_hres() == spec.hres
-            and lib.crtx_nes_border() == int(spec.border)), "variant mismatch"
+            and lib.crtx_nes_border() == int(spec.border)
+            and lib.crtx_do_vsync() == int(spec.do_vsync) and lib.crtx_do_hsync() == int(spec.do_hsync)), "variant mismatch"
     _libs[variant] = lib
     return lib
 

@@ -280,13 +280,16 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
             w0 = (pos - start4) >> 2;      // row word the vector's first word is (-3 .. nw)
             return row;
         };
+        // CRT_DO_VSYNC 0: the candidates are searched in analog[], before any noise (crt_core.c:323-337); heads keep it
+        auto raw_cand = [&](int idx) { return !kDoVsync && idx >= kHeadLines * kHeadVecs; };
         uint4 v[kStageBatch];
 #pragma unroll
         for (int b = 0; b < kStageBatch; b++) {
             int pos, w0, nw;
             (void) place(b * kSyncThreads + tid, pos, w0, nw);
             v[b] = make_uint4(0u, 0u, 0u, 0u);
-            if (nw > 0 && pos >= 0) v[b] = __ldg(reinterpret_cast<const uint4 *>(from + pos));
+            const signed char *src = raw_cand(b * kSyncThreads + tid) ? analog : from;
+            if (nw > 0 && pos >= 0) v[b] = __ldg(reinterpret_cast<const uint4 *>(src + pos));
         }
 #pragma unroll
         for (int b = 0; b < kStageBatch; b++) {
@@ -294,7 +297,7 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
             unsigned *row = place(b * kSyncThreads + tid, pos, w0, nw);
             if (nw == 0) continue;
             unsigned w[4] = { v[b].x, v[b].y, v[b].z, v[b].w };
-            if (kFusedNoise && pos >= 0) {
+            if (kFusedNoise && pos >= 0 && !raw_cand(b * kSyncThreads + tid)) {
                 if (noise == 0 && pos + 16 <= kInputSize) {
 #pragma unroll
                     for (int e = 0; e < 4; e++) w[e] = clamp127_4(w[e]);
@@ -343,6 +346,7 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
             break;
         }
     }
+    if (!kDoVsync) vs = -3; // crt_core.c:341: the search only gave the field
     int field = (jcross > kHres / 2);
     const int ratio = (((cfg.outh << 16) / kLines) + 32768) >> 16; // crt_core.c:404-407
     field *= ratio / 2;
@@ -382,7 +386,21 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
     // is evaluated in parallel from the current guess of its predecessor; a sweep that changes nothing
     // proves hs[] is the chain's unique solution.  The sync edge recaptures the search from any start
     // within the window, so this takes a handful of sweeps instead of 240 dependent steps.
-    for (int sweep = 0; sweep <= kLines; sweep++) {
+    // CRT_DO_HSYNC 0 (crt_core.c:446-450): the search's result is dropped and hsync is 0 after every decoded line.  A skipped
+    // line keeps its predecessor's, so hs_in lasts until the first decoded line; warp 0 finds it with ballots, no sweeps.
+    if (!kDoHsync) {
+        if (warp == 0) {
+            bool seen = false;
+            for (int k0 = 0; k0 < kLines; k0 += 32) {
+                const int k = k0 + lane;
+                const unsigned dec = __ballot_sync(0xffffffffu, k < kLines && sh.ln[k].beg >= 0);
+                if (k < kLines && (seen || (dec & (0xffffffffu >> (31 - lane))) != 0)) sh.hs[k] = 0;
+                seen = seen || dec != 0;
+            }
+        }
+        __syncthreads();
+    }
+    for (int sweep = 0; kDoHsync && sweep <= kLines; sweep++) {
         int nh[(kLines + kSyncThreads - 1) / kSyncThreads];
         int changed = 0;
 #pragma unroll

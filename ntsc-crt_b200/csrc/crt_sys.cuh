@@ -62,6 +62,10 @@ static_assert(!kConv || CRT_CC_SAMPLES == 4, "CRTX_CONV: the reference disables 
 // CRT_DO_BLOOM 1 (crt_core.h:70): the decoder derives each line's width from a filtered beam energy
 // (crt_core.c:399-402, 512-526) and the encoders shrink the picture (crt_ntsc.c:148-160)
 constexpr bool kBloom = (CRT_DO_BLOOM != 0);
+// CRT_DO_VSYNC 0 (crt_core.h:71): k_sync takes the field from analog[] before the noise and decodes from vsync -3
+// (crt_core.c:323-342).  CRT_DO_HSYNC 0 (crt_core.h:72): hsync is 0 after every decoded line (crt_core.c:446-450).
+constexpr bool kDoVsync = (CRT_DO_VSYNC != 0);
+constexpr bool kDoHsync = (CRT_DO_HSYNC != 0);
 
 constexpr int kHres = CRT_HRES;
 constexpr int kVres = CRT_VRES;

@@ -736,6 +736,8 @@ const char *crtx_last_error(void) { return g_error; }
 int crtx_system(void) { return kSystem; }
 int crtx_chroma_pattern(void) { return kPattern; }
 int crtx_nes_border(void) { return kNesBorder ? 1 : 0; }
+int crtx_do_vsync(void) { return kDoVsync ? 1 : 0; }
+int crtx_do_hsync(void) { return kDoHsync ? 1 : 0; }
 int crtx_hres(void) { return kHres; }
 int crtx_input_size(void) { return kInputSize; }
 int crtx_lines(void) { return kLines; }

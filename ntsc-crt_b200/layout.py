@@ -9,7 +9,7 @@ views are used for the product libraries (ntsc-crt_b200/lib) and, in the tests, 
 compiled reference (oracle/_ref), which is how layout identity is checked.
 """
 import ctypes as C
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 
 PIX_RGB, PIX_BGR, PIX_ARGB, PIX_RGBA, PIX_ABGR, PIX_BGRA = range(6)  # crt_core.h:62-67
 
@@ -27,7 +27,7 @@ def bpp4fmt(fmt):
 
 @dataclass(frozen=True)
 class SystemSpec:
-    name: str          # library suffix: ntsc | ntsc_conv[6|5|4] | vhs | nes | nes_p0 | nes_border | snes | ...
+    name: str          # library suffix: ntsc | ntsc_conv[6|5|4] | vhs | nes | nes_p0 | nes_border | snes | ntsc_nosync | ...
     system: int        # CRT_SYSTEM
     pattern: int       # CRT_CHROMA_PATTERN
     hres: int
@@ -47,6 +47,8 @@ class SystemSpec:
     black: int
     sync: int
     border: bool = False  # NES_BORDER 1 (crt_nes.c:64-69): the NES encoder draws settings.border_color
+    do_vsync: bool = True  # CRT_DO_VSYNC (crt_core.h:71); off: field from analog[] before the noise, vsync -3
+    do_hsync: bool = True  # CRT_DO_HSYNC (crt_core.h:72); off: hsync 0 after every decoded line
 
     @property
     def input_size(self):
@@ -128,8 +130,25 @@ SPECS = {
 }
 
 
+# The sync switches of crt_core.h:71-72 go with every system: `<stock variant><suffix>` names its build with them off
+# (capi.SYNC_VARIANTS are built as libraries, the other combinations through `make custom`).  Not combined with the
+# convolution decoder or bloom.
+SYNC_SUFFIXES = {"_novsync": (False, True), "_nohsync": (True, False), "_nosync": (False, False)}
+_sync_specs = {}
+
+
 def system_spec(name):
-    return SPECS[name]
+    if name in SPECS:
+        return SPECS[name]
+    if name not in _sync_specs:
+        for suffix, (do_vsync, do_hsync) in SYNC_SUFFIXES.items():
+            base = name[:-len(suffix)]
+            if name.endswith(suffix) and base in SPECS and not uses_convolution(base) and not base.endswith("_bloom"):
+                _sync_specs[name] = replace(SPECS[base], name=name, do_vsync=do_vsync, do_hsync=do_hsync)
+                break
+        else:
+            raise KeyError(name)
+    return _sync_specs[name]
 
 
 def conv_taps(name):

@@ -6,6 +6,7 @@ cd "$(dirname "$0")/.."
 make -s -C ntsc-crt_b200/csrc -j8 all > /dev/null
 make -s -C oracle all > /dev/null
 make -s -C oracle -f nes_border.mk all > /dev/null
+make -s -C oracle -f sync.mk all > /dev/null
 make -s -C tools all > /dev/null
 python - <<'P'
 import pkgload; pkgload.load()
