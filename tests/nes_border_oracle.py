@@ -11,9 +11,8 @@ tests/test_oracle_nes_border.py.
 import numpy as np
 
 import support as S
-from ntsc_crt_b200 import capi, layout
+from ntsc_crt_b200 import layout
 
-BORDER_VARIANTS = list(capi.BORDER_VARIANTS)
 # the largest xoffset that keeps the picture inside its line: xo = (AV_BEG + xoffset) & ~3, xo + AV_LEN <= CRT_HRES
 XMAX = {"nes_border": 30, "nes_p0_border": 34}
 # every 9-bit border colour, and colours with bits above bit 8 (square_sample reads bits 0-8 only)
@@ -101,7 +100,3 @@ class BorderOracleEngine(S.OracleEngine):
             keep = ~drawn[n * H + lb:(n + 1) * H]
             analog[n * H + lb:(n + 1) * H][keep] = row[keep]
 
-
-def oracle_engine(variant, *a, **kw):
-    """the CPU model of any NES variant: BorderOracleEngine for the border builds, support.OracleEngine otherwise"""
-    return (BorderOracleEngine if layout.system_spec(variant).border else S.OracleEngine)(variant, *a, **kw)

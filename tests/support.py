@@ -185,7 +185,8 @@ class CEngine:
 # ----------------------------------------------------------------------------------
 # A checkout without the reference sources has no oracle/_ref.  The comparisons with the reference still run there:
 # tests/golden/ref_states.json holds, per test and in call order, digests of every reference state the test compares
-# and every value it probes from a reference build.  Where oracle/_ref exists the reference itself is used, and
+# and every value it probes from a reference build.  Where oracle/_ref exists the reference itself is used and must
+# still give the recorded values, and
 #     CRT_RECORD_REF=1 python -m pytest tests/<file>.py
 # rewrites the records of the tests it runs.
 
@@ -224,11 +225,18 @@ def _save_records():
 
 
 def _record(value):
+    """a value the live reference gave: recorded with CRT_RECORD_REF=1, else checked against its record where the test
+    has one"""
+    tid = _test_id()
     if RECORD:
         if not _recorded_now:
             atexit.register(_save_records)
-        tid = _test_id()
         _recorded_now.setdefault(tid, []).append(value)  # (replaces what the file held for this test)
+    elif tid in _load_records():
+        k = _cursor.get(tid, 0)
+        want = _replay()
+        assert json.loads(json.dumps(value)) == want, (
+            "%s: the reference gave %r as value #%d, its record in %s is %r" % (tid, value, k, REF_STATES, want))
     return value
 
 
@@ -237,7 +245,7 @@ def _replay():
     recs = _load_records().get(tid)
     k = _cursor.get(tid, 0)
     assert recs is not None and k < len(recs), (
-        "%s: no recorded reference value #%d in %s (oracle/_ref is not built here)" % (tid, k, REF_STATES))
+        "%s: no recorded reference value #%d in %s" % (tid, k, REF_STATES))
     _cursor[tid] = k + 1
     return recs[k]
 
@@ -260,7 +268,7 @@ def end_reference_scope():
 
 def from_reference(path, compute):
     """compute(path) where the reference build `path` (under oracle/_ref) exists, else the value it gave when recorded.
-    The value must be JSON data: probe large outputs through digest()."""
+    The value must be JSON data: probe large outputs through digest().  A live value must equal its record."""
     if os.path.exists(path):
         return _record(compute(path))
     return _replay()
@@ -526,6 +534,29 @@ class OracleEngine:
                     hsync=self.hsync, vsync=self.vsync, rn=self.rn)
 
 
+def oracle_engine(variant, outw, outh, fmt=layout.PIX_BGRA, seed=1):
+    """the CPU model of any variant: nes_border_oracle.BorderOracleEngine for the NES_BORDER 1 builds,
+    sync_oracle.SyncOracleEngine where a sync search is off, OracleEngine otherwise"""
+    spec = layout.system_spec(variant)
+    if spec.border:
+        from nes_border_oracle import BorderOracleEngine as model  # (those modules import this one)
+    elif not (spec.do_vsync and spec.do_hsync):
+        from sync_oracle import SyncOracleEngine as model
+    else:
+        model = OracleEngine
+    return model(variant, outw, outh, fmt, seed=seed)
+
+
+def oracle_settings(system, settings):
+    """a capi.Batch source's settings as the CPU model takes them: the batch's `reinit` is the NES and NES-RGB
+    oracles' field_initialized = not reinit; the other oracles have no such setting"""
+    kw = dict(settings)
+    reinit = kw.pop("reinit", None)
+    if reinit is not None and system in (layout.SYS_NES, layout.SYS_NESRGB):
+        kw["field_initialized"] = int(not reinit)
+    return kw
+
+
 def assert_same_state(a, b, what=""):
     """Bit-exact comparison of two engine states with a useful first-mismatch report.  `a` may be a reference state,
     live or recorded (see RefEngine)."""
@@ -580,11 +611,10 @@ class ProductEngine(CEngine):
 # the drop-in interface: the product, the oracle and the reference through the same calls
 # ----------------------------------------------------------------------------------
 
-def trio(variant, outw, outh, fmt=layout.PIX_BGRA, oracle=OracleEngine):
-    """(product, CPU model, reference or None where it is not built), each with an outw x outh monitor;
-    oracle(variant, outw, outh, fmt) makes the CPU model (nes_border_oracle.oracle_engine for the border builds)"""
+def trio(variant, outw, outh, fmt=layout.PIX_BGRA):
+    """(product, CPU model, reference or None where it is not built), each with an outw x outh monitor"""
     gpu = ProductEngine(variant, outw, outh, fmt)
-    ora = oracle(variant, outw, outh, fmt)
+    ora = oracle_engine(variant, outw, outh, fmt)
     ref = RefEngine(variant, outw, outh, fmt, seed=1) if have_ref(variant) else None
     return gpu, ora, ref
 
@@ -620,10 +650,9 @@ class BatchRig:
     """A capi.Batch and one CPU model per monitor, driven through the same calls and compared whole state by whole state.
 
     mons[i] = dict(outw, outh, fmt, noise, knobs), and optionally seed: the VHS rand() seed of both sides.  options:
-    (name, value) pairs set on the batch first.  oracle(variant, outw, outh, fmt, seed=...) makes one monitor's CPU
-    model (nes_border_oracle.oracle_engine for the border builds)."""
+    (name, value) pairs set on the batch first."""
 
-    def __init__(self, variant, mons, options=(), oracle=OracleEngine):
+    def __init__(self, variant, mons, options=()):
         import torch
         from ntsc_crt_b200 import capi
         self.mons = mons
@@ -636,7 +665,7 @@ class BatchRig:
             self.b.set_monitor(i, out, fmt=m["fmt"], noise=m["noise"], **m["knobs"])
             if "seed" in m:
                 self.b.seed(m["seed"], first=i, count=1)
-            o = oracle(variant, m["outw"], m["outh"], m["fmt"], seed=m.get("seed", 1))
+            o = oracle_engine(variant, m["outw"], m["outh"], m["fmt"], seed=m.get("seed", 1))
             o.set(**m["knobs"])
             self.outs.append(out)
             self.oras.append(o)
@@ -650,14 +679,9 @@ class BatchRig:
         return self._dev[id(img)][1]
 
     def source(self, i, img, **settings):
-        """monitor i's next source image (numpy) and settings, on both sides.  The batch's `reinit` is the NES and NES-RGB
-        oracles' field_initialized = not reinit; the other oracles have no such setting."""
-        kw = dict(settings)
-        reinit = kw.pop("reinit", None)
-        if reinit is not None and self.b.spec.system in (layout.SYS_NES, layout.SYS_NESRGB):
-            kw["field_initialized"] = int(not reinit)
+        """monitor i's next source image (numpy) and settings, on both sides (oracle_settings)"""
         self.b.set_source(i, self._device(img), **settings)
-        self._src[i] = (img, kw)
+        self._src[i] = (img, oracle_settings(self.b.spec.system, settings))
 
     def modulate(self, first=0, count=None):
         count = len(self.mons) - first if count is None else count
@@ -694,6 +718,71 @@ class BatchRig:
 
     def close(self):
         self.b.close()
+
+
+def written_rows(lines, outh, scanlines):
+    """the output rows a field's decoded lines (capi.Batch.get_lines) write, as a mask of outh rows: from each line's
+    beg on, max(1, end - scanlines - beg) of them (rows_written, crt_sync.cuh)"""
+    rows = np.zeros(outh, dtype=bool)
+    for l in lines:
+        if l.beg >= 0:
+            rows[l.beg:l.beg + max(1, l.end - scanlines - l.beg)] = True
+    return rows
+
+
+def _rgb_fields(it):
+    return rand_image(320, 240, seed=11), dict(format=layout.PIX_BGRA, as_color=1, field=it & 1, frame=(it >> 1) & 1)
+
+
+def decode_in_blocks(variant, outw, outh, world, source=_rgb_fields, fields=6, noise=4, scanlines=1, blend=1, v_fac=0):
+    """The scanline-block partition of one image (SURVEY 8e): `world` contexts stand in for as many ranks, each decoding
+    its own block of lines of every field (crtx_set_option line_lo / line_hi) into its own image, with the rows handed
+    over by the rules of ntsc_crt_b200.sharding.ImageSharder.  The merged image must equal the CPU model's sequential
+    decode.  source(it) -> (numpy image, batch settings) of field `it` (oracle_settings for the model); by default an RGB
+    picture with interlaced fields."""
+    import torch
+    from ntsc_crt_b200 import capi, sharding
+    ora = oracle_engine(variant, outw, outh)
+    ora.set(blend=blend, scanlines=scanlines, v_fac=v_fac)
+    ranks = []
+    for r in range(world):
+        b = capi.Batch(variant, 1)
+        if b.spec.system == layout.SYS_VHS:
+            b.seed(1, first=0, count=1)  # (the oracle's rand() replica is seeded with 1)
+        out = torch.zeros(outh, outw, 4, dtype=torch.uint8, device="cuda")
+        b.set_monitor(0, out, fmt=layout.PIX_BGRA, noise=noise, blend=blend, scanlines=scanlines, v_fac=v_fac)
+        b.commit_monitors()
+        part = sharding.ImageSharder(out, b.spec.lines, rank=r, world=world, v_fac=v_fac)
+        part.apply(b)
+        ranks.append((b, out, part))
+    for it in range(fields):
+        img, kw = source(it)
+        dimg = torch.from_numpy(img.view(np.int16) if img.dtype == np.uint16 else img).cuda()
+        ora.modulate(img, **oracle_settings(ora.spec.system, kw))
+        ora.demodulate(noise)
+        ends = []
+        for r in range(world - 1):  # what ImageSharder.fetch_halo_rows does over the process group, before the field
+            (_, dst, ps), (_, src, pn) = ranks[r], ranks[r + 1]
+            cnt = ps._halo_count(r)
+            if cnt:
+                dst[ps.r1:ps.r1 + cnt].copy_(src[pn.r0:pn.r0 + cnt])
+        for b, out, part in ranks:
+            b.set_source(0, dimg, **kw)
+            b.modulate()
+            b.demodulate()
+            last = b.get_lines(0)[part.hi - 1]
+            ends.append(0 if last.beg < 0 else max(last.beg + 1, last.end - scanlines))
+        torch.cuda.synchronize()
+        for r in range(world - 1):  # what ImageSharder.exchange_spill_rows does over the process group
+            (_, src, ps), (_, dst, pd) = ranks[r], ranks[r + 1]
+            cnt = max(0, min(ends[r], outh, ps.r1 + ps.max_spill()) - ps.r1)
+            if cnt and pd.r0 == ps.r1:
+                dst[pd.r0:pd.r0 + cnt].copy_(src[ps.r1:ps.r1 + cnt])
+    full = np.zeros((outh, outw, 4), dtype=np.uint8)
+    for b, out, part in ranks:
+        full[part.r0:part.r1] = out[part.r0:part.r1].cpu().numpy()
+        b.close()
+    assert np.array_equal(full, ora.out), diff_report("merged image", full, ora.out)
 
 
 # ----------------------------------------------------------------------------------

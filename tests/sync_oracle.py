@@ -8,7 +8,7 @@ The switches change only the sync pre-pass of crt_demodulate:
   * CRT_DO_HSYNC 0 (crt_core.c:446-450): the hsync search still runs but its result is dropped: hsync is 0 after every
     decoded line.  The search has no side effect, so the model does not run it.
 SyncOracleEngine runs support.OracleEngine's encoders, noise pass and line pass and does this sync pass itself, in the
-oracle's 32-bit arithmetic.  It is pinned against the reference built with the switches off (oracle/sync.mk) by
+oracle's 32-bit arithmetic.  It is pinned against the reference built with the switches off (oracle/Makefile) by
 tests/test_oracle_sync_switches.py.
 """
 import ctypes as C
@@ -16,9 +16,7 @@ import ctypes as C
 import numpy as np
 
 import support as S
-from ntsc_crt_b200 import capi, layout
 
-SYNC_VARIANTS = list(capi.SYNC_VARIANTS)
 # every system of the reference, under the name of its stock library, and the three switch sets (layout.SYNC_SUFFIXES)
 SYSTEMS = ("ntsc", "vhs", "nes", "snes", "nesrgb", "template", "pv1k")
 SWITCHES = ("novsync", "nohsync", "nosync")
@@ -148,8 +146,3 @@ class SyncOracleEngine(S.OracleEngine):
                     ang += 360 // CC
         return field, table
 
-
-def oracle_engine(variant, *a, **kw):
-    """the CPU model of any variant: SyncOracleEngine where a sync switch is off, support.OracleEngine otherwise"""
-    spec = layout.system_spec(variant)
-    return (S.OracleEngine if spec.do_vsync and spec.do_hsync else SyncOracleEngine)(variant, *a, **kw)

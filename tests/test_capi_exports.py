@@ -1,6 +1,6 @@
 """CPU-side checks of the boundary: every symbol include/*.h declares is exported by every
-library variant, struct layouts equal the reference's, and the host-only entry points
-(crt_bpp4fmt, crt_sincos14) agree with the oracle.  No compute calls: there is no GPU here."""
+library variant, every library reports the build its variant names, struct layouts equal the reference's, and the
+host-only entry points (crt_bpp4fmt, crt_sincos14) agree with the oracle.  No compute calls: there is no GPU here."""
 import ctypes as C
 import os
 import re
@@ -19,7 +19,7 @@ def declared(header):
     return sorted(set(re.findall(r"\b(crtx?_[a-z0-9_]+)\s*\(", text)))
 
 
-@pytest.mark.parametrize("variant", capi.VARIANTS)
+@pytest.mark.parametrize("variant", capi.ALL_VARIANTS)
 def test_every_declared_symbol_is_exported(variant):
     if not os.path.exists(capi.lib_path(variant)):
         pytest.fail("library not built: run __graft_entry__.build()")
@@ -30,13 +30,28 @@ def test_every_declared_symbol_is_exported(variant):
         assert hasattr(lib, name), "%s missing from %s" % (name, variant)
 
 
-@pytest.mark.parametrize("variant", capi.VARIANTS)
+def test_variant_groups_are_disjoint():
+    """the stock builds, the border builds and the sync-switch builds are three separate groups, ALL_VARIANTS all three,
+    and each variant's spec puts it in its group"""
+    assert capi.ALL_VARIANTS == capi.VARIANTS + capi.BORDER_VARIANTS + capi.SYNC_VARIANTS
+    assert len(set(capi.ALL_VARIANTS)) == len(capi.ALL_VARIANTS)
+    for variant in capi.ALL_VARIANTS:
+        spec = layout.system_spec(variant)
+        group = (capi.BORDER_VARIANTS if spec.border else capi.VARIANTS if spec.do_vsync and spec.do_hsync
+                 else capi.SYNC_VARIANTS)
+        assert variant in group, variant
+
+
+@pytest.mark.parametrize("variant", capi.ALL_VARIANTS)
 def test_geometry_and_host_only_entry_points(variant):
+    """the library reports its system, timing, border switch and sync switches as its variant's spec has them (every
+    stock library: no border, both sync searches on)"""
     lib = capi.load(variant)
     spec = layout.system_spec(variant)
     assert (lib.crtx_system(), lib.crtx_chroma_pattern(), lib.crtx_hres(), lib.crtx_input_size(),
-            lib.crtx_lines(), lib.crtx_cc_vper()) == (spec.system, spec.pattern, spec.hres,
-                                                      spec.input_size, spec.lines, spec.vper)
+            lib.crtx_lines(), lib.crtx_cc_vper(), lib.crtx_nes_border(), lib.crtx_do_vsync(), lib.crtx_do_hsync()) == (
+        spec.system, spec.pattern, spec.hres, spec.input_size, spec.lines, spec.vper, int(spec.border),
+        int(spec.do_vsync), int(spec.do_hsync))
     ora = S.oracle_lib()
     s1, c1, s2, c2 = C.c_int(), C.c_int(), C.c_int(), C.c_int()
     for n in range(-17000, 34000, 13):

@@ -172,9 +172,7 @@ def test_frames_host_moves_only_the_rows_a_field_touches(variant, raw, monkeypat
                 if not host_rows:
                     assert np.array_equal(got, oras[i].out), "%s field %d monitor %d: %s" % (variant, it, i, S.diff_report("host image", got, oras[i].out))
                     continue
-                for l in b.get_lines(i):
-                    if l.beg >= 0:
-                        written[i][l.beg:l.beg + max(1, l.end - 1 - l.beg)] = True
+                written[i] |= S.written_rows(b.get_lines(i), outh, 1)
                 w = written[i]
                 assert 0 < w.sum() < outh or it > 0
                 assert np.array_equal(got[w], oras[i].out[w]), "%s field %d monitor %d: %s" % (

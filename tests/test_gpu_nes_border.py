@@ -2,7 +2,7 @@
 stock timing, libcrt_b200_nes_p0_border.so on chroma pattern 0) draw lines CRT_TOP .. CRT_BOT + 2 from LAV_BEG on in
 settings.border_color on every call, the picture over it (crt_nes.c:138-161).  Every field is compared bit for bit with
 the CPU model of the border (tests/nes_border_oracle.py, the stock oracle plus the border bytes) and, where it is built,
-with the reference compiled with the switch on (oracle/_ref/libref_*_border.so, oracle/nes_border.mk):
+with the reference compiled with the switch on (oracle/_ref/libref_*_border.so, oracle/Makefile):
 batches that span the border colours, dot crawl, black and white points, picture offsets and re-initialisations; the
 drop-in interface; crtx_frames_host; a line-block split.  The stock NES library ignores the field, as the reference does.
 
@@ -11,8 +11,8 @@ import numpy as np
 import pytest
 
 import support as S
-from nes_border_oracle import BORDER_VARIANTS, COLOURS, XMAX, oracle_engine
-from ntsc_crt_b200 import capi, layout, sharding
+from nes_border_oracle import COLOURS, XMAX
+from ntsc_crt_b200 import capi, layout
 from test_simt_kernels import simt_libs  # noqa: F401  (session fixture of the interpreter builds)
 import test_simt_kernels as _simt
 
@@ -41,7 +41,7 @@ def check_batch(variant, n=None, fields=None):
         bp, wp, hue, blend, scan = KNOBS[i % len(KNOBS)]
         mons.append(dict(outw=OUTW, outh=OUTH, fmt=layout.PIX_BGRA, noise=(5 * i) % 17,
                          knobs=dict(blend=blend, scanlines=scan, black_point=bp, white_point=wp, hue=hue)))
-    rig = S.BatchRig(variant, mons, oracle=oracle_engine)
+    rig = S.BatchRig(variant, mons)
     imgs = [S.nes_image(seed=300 + i, rainbow=(i % 5 == 4)) for i in range(n)]
     for it in range(fields):
         for i in range(n):
@@ -55,7 +55,7 @@ def check_batch(variant, n=None, fields=None):
 def check_dropin(variant, fields=8):
     """the drop-in interface (crt_modulate / crt_demodulate, NTSC_SETTINGS.border_color), after every call; the settings
     are re-initialised once more half way"""
-    gpu, ora, ref = S.trio(variant, 832, 624, oracle=oracle_engine)
+    gpu, ora, ref = S.trio(variant, 832, 624)
     S.run_all((gpu, ora, ref), lambda e: e.set(blend=1, scanlines=1, black_point=3, white_point=93))
     img = S.nes_image(seed=21)
     for it in range(fields):
@@ -75,8 +75,7 @@ def check_frames_host(variant, n=3, fields=4):
     import torch
     outw, outh = 640, 480
     rig = S.BatchRig(variant, [dict(outw=outw, outh=outh, fmt=layout.PIX_BGRA, noise=2 + i,
-                                    knobs=dict(blend=1, scanlines=1, black_point=i, white_point=100 - 5 * i)) for i in range(n)],
-                     oracle=oracle_engine)
+                                    knobs=dict(blend=1, scanlines=1, black_point=i, white_point=100 - 5 * i)) for i in range(n)])
     host = [torch.zeros(outh, outw, 4, dtype=torch.uint8).pin_memory() for _ in range(n)]
     srcs = [torch.from_numpy(S.nes_image(256, 240 - 16 * i, seed=60 + i).astype(np.int16)).pin_memory() for i in range(n)]
     imgs = [s.numpy().view(np.uint16) for s in srcs]  # (the page-locked images themselves)
@@ -89,60 +88,19 @@ def check_frames_host(variant, n=3, fields=4):
         rig.check("%s frames_host field %d" % (variant, it))
         for i in range(n):
             got, want = host[i].numpy(), rig.oras[i].out
-            rows = np.zeros(outh, dtype=bool)
-            for l in rig.b.get_lines(i):
-                if l.beg >= 0:
-                    rows[l.beg:l.beg + max(1, l.end - 1 - l.beg)] = True
+            rows = S.written_rows(rig.b.get_lines(i), outh, 1)
             assert rows.any()
             assert np.array_equal(got[rows], want[rows]), (variant, it, i, S.diff_report("rows", got[rows], want[rows]))
     rig.close()
 
 
-def check_line_blocks(variant, world=2, outw=832, outh=624, fields=5):
-    """two contexts each decode their own block of lines (crtx_set_option line_lo / line_hi, sharding.ImageSharder);
-    the merged image equals the oracle's sequential decode"""
-    import torch
+def check_line_blocks(variant, outw=832, outh=624, fields=5):
+    """two contexts each decode their own block of lines (support.decode_in_blocks), the border colour, dot crawl and
+    picture offsets changing from field to field"""
     img = S.nes_image(seed=77)
-    dimg = torch.from_numpy(img.astype(np.int16)).cuda()
-    ora = oracle_engine(variant, outw, outh)
-    ora.set(blend=1, scanlines=1)
-    ranks = []
-    for r in range(world):
-        b = capi.Batch(variant, 1)
-        out = torch.zeros(outh, outw, 4, dtype=torch.uint8, device="cuda")
-        b.set_monitor(0, out, fmt=layout.PIX_BGRA, noise=4, blend=1, scanlines=1)
-        b.commit_monitors()
-        part = sharding.ImageSharder(out, b.spec.lines, rank=r, world=world)
-        part.apply(b)
-        ranks.append((b, out, part))
-    for it in range(fields):
-        kw = dict(dot_crawl_offset=it % 3, border_color=(0x22 * (it + 1)) & 0x1ff, xoffset=4 * it, yoffset=it)
-        ora.modulate(img, field_initialized=int(it != 0), **kw)
-        ora.demodulate(4)
-        ends = []
-        for r in range(world - 1):  # the halo rows ImageSharder.fetch_halo_rows hands over before the field
-            (_, dst, ps), (_, src, pn) = ranks[r], ranks[r + 1]
-            cnt = ps._halo_count(r)
-            if cnt:
-                dst[ps.r1:ps.r1 + cnt].copy_(src[pn.r0:pn.r0 + cnt])
-        for b, out, part in ranks:
-            b.set_source(0, dimg, **kw)
-            b.sources[0].reinit = int(it == 0)
-            b.modulate()
-            b.demodulate()
-            last = b.get_lines(0)[part.hi - 1]
-            ends.append(0 if last.beg < 0 else max(last.beg + 1, last.end - 1))
-        torch.cuda.synchronize()
-        for r in range(world - 1):  # the spill rows ImageSharder.exchange_spill_rows hands on after it
-            (_, src, ps), (_, dst, pd) = ranks[r], ranks[r + 1]
-            cnt = max(0, min(ends[r], outh, ps.r1 + ps.max_spill()) - ps.r1)
-            if cnt and pd.r0 == ps.r1:
-                dst[pd.r0:pd.r0 + cnt].copy_(src[ps.r1:ps.r1 + cnt])
-    full = np.zeros((outh, outw, 4), dtype=np.uint8)
-    for b, out, part in ranks:
-        full[part.r0:part.r1] = out[part.r0:part.r1].cpu().numpy()
-        b.close()
-    assert np.array_equal(full, ora.out), S.diff_report("merged image", full, ora.out)
+    S.decode_in_blocks(variant, outw, outh, 2, lambda it: (img, dict(
+        reinit=int(it == 0), dot_crawl_offset=it % 3, border_color=(0x22 * (it + 1)) & 0x1ff, xoffset=4 * it, yoffset=it)),
+        fields=fields)
 
 
 def check_stock_ignores_the_border(variant="nes", fields=3):
@@ -155,7 +113,7 @@ def check_stock_ignores_the_border(variant="nes", fields=3):
         b.set_monitor(i, outs[i], fmt=layout.PIX_BGRA, noise=3, blend=1, scanlines=1)
     b.commit_monitors()
     dimg = torch.from_numpy(S.nes_image(seed=8).astype(np.int16)).cuda()
-    ora = oracle_engine(variant, 320, 240)
+    ora = S.oracle_engine(variant, 320, 240)
     ora.set(blend=1, scanlines=1)
     for it in range(fields):
         for i in range(2):
@@ -184,25 +142,25 @@ def check_stock_ignores_the_border(variant="nes", fields=3):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", BORDER_VARIANTS)
+@pytest.mark.parametrize("variant", capi.BORDER_VARIANTS)
 def test_batch_spans_border_colours_offsets_and_reinit(variant):
     check_batch(variant)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", BORDER_VARIANTS)
+@pytest.mark.parametrize("variant", capi.BORDER_VARIANTS)
 def test_dropin_border(variant):
     check_dropin(variant)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", BORDER_VARIANTS)
+@pytest.mark.parametrize("variant", capi.BORDER_VARIANTS)
 def test_frames_host_border(variant):
     check_frames_host(variant)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", BORDER_VARIANTS)
+@pytest.mark.parametrize("variant", capi.BORDER_VARIANTS)
 def test_line_blocks_border(variant):
     check_line_blocks(variant)
 
@@ -212,32 +170,15 @@ def test_stock_nes_ignores_border_color():
     check_stock_ignores_the_border()
 
 
-@pytest.mark.parametrize("variant", BORDER_VARIANTS)
-def test_border_library_exports_and_geometry(variant):
-    """every symbol the headers declare is exported, and the library reports its system, timing and border switch
-    (capi.load checks crtx_nes_border against the variant too)"""
-    import ctypes as C
-    import test_capi_exports as X
-    lib = C.CDLL(capi.lib_path(variant))
-    for name in X.declared("crt_b200.h") + X.declared("crtx_batch.h"):
-        assert hasattr(lib, name), "%s missing from %s" % (name, variant)
-    lib = capi.load(variant)
-    spec = layout.system_spec(variant)
-    assert (lib.crtx_system(), lib.crtx_chroma_pattern(), lib.crtx_hres(), lib.crtx_nes_border()) == (
-        layout.SYS_NES, spec.pattern, spec.hres, 1)
-    assert capi.load("nes").crtx_nes_border() == 0 and capi.load("nes_p0").crtx_nes_border() == 0
-    assert variant in capi.ALL_VARIANTS and variant not in capi.VARIANTS
-
-
 # ---- the same bodies on the CPU, through the SIMT interpreter ------------------------------------------------------
 class TestOnTheInterpreter:
     simt_backend = staticmethod(_simt.simt_backend)  # autouse within this class: the interpreter builds, host "device" tensors
 
-    @pytest.mark.parametrize("variant", BORDER_VARIANTS)
+    @pytest.mark.parametrize("variant", capi.BORDER_VARIANTS)
     def test_batch(self, variant):
         check_batch(variant, n=6, fields=7)
 
-    @pytest.mark.parametrize("variant", BORDER_VARIANTS)
+    @pytest.mark.parametrize("variant", capi.BORDER_VARIANTS)
     def test_every_border_colour(self, variant):
         """every colour of COLOURS through the interpreted encoder: analog only, 16 monitors per call"""
         import torch
@@ -247,7 +188,7 @@ class TestOnTheInterpreter:
         for i in range(n):
             bp, wp, hue, blend, scan = KNOBS[i % len(KNOBS)]
             b.set_monitor(i, torch.zeros(48, 64, 4, dtype=torch.uint8), fmt=layout.PIX_BGRA, black_point=bp, white_point=wp)
-            o = oracle_engine(variant, 64, 48)
+            o = S.oracle_engine(variant, 64, 48)
             o.set(black_point=bp, white_point=wp)
             oras.append(o)
         b.commit_monitors()
@@ -265,11 +206,11 @@ class TestOnTheInterpreter:
                 assert np.array_equal(got, oras[i].analog), (variant, it, i, S.diff_report("analog", got, oras[i].analog))
         b.close()
 
-    @pytest.mark.parametrize("variant", BORDER_VARIANTS)
+    @pytest.mark.parametrize("variant", capi.BORDER_VARIANTS)
     def test_dropin(self, variant):
         check_dropin(variant, fields=4)
 
-    @pytest.mark.parametrize("variant", BORDER_VARIANTS)
+    @pytest.mark.parametrize("variant", capi.BORDER_VARIANTS)
     def test_frames_host(self, variant, monkeypatch):
         monkeypatch.setenv("SIMT_HOST_MAPPED", "1")  # (only the interpreter build of the library reads this)
         check_frames_host(variant, n=2, fields=3)

@@ -271,9 +271,7 @@ def check_frames_host(variant, host_src):
             got, padding = full[:, :outw * 4].reshape(outh, outw, 4), full[:, outw * 4:]
             assert (padding == SENT).all(), (variant, host_src, it, i)
             assert np.array_equal(outs[i].cpu().numpy().reshape(outh, opitch)[:, :outw * 4].reshape(outh, outw, 4), oras[i].out)
-            for l in b.get_lines(i):
-                if l.beg >= 0:
-                    written[i][l.beg:l.beg + max(1, l.end - 1 - l.beg)] = True
+            written[i] |= S.written_rows(b.get_lines(i), outh, 1)
             w = written[i]
             assert 0 < w.sum() < outh or it > 0
             assert np.array_equal(got[w], oras[i].out[w]), (variant, host_src, it, i, S.diff_report("rows", got[w], oras[i].out[w]))

@@ -3,7 +3,7 @@
 and the lines are decoded from vsync -3 (crt_core.c:323-342); with the hsync search off hsync is 0 after every decoded
 line (crt_core.c:446-450).  Every field is compared bit for bit with the CPU model of the switches (tests/sync_oracle.py,
 the stock oracle with its own sync pass) and, where it is built, with the reference compiled with the switches off
-(oracle/_ref/libref_*_no*sync.so, oracle/sync.mk): mixed batches with noise up to 255, geometries on k_lines2 and on
+(oracle/_ref/libref_*_no*sync.so, oracle/Makefile): mixed batches with noise up to 255, geometries on k_lines2 and on
 k_lines, the generic equaliser and poked sync states; the drop-in interface; crtx_frames_host; a line-block split; the
 reference's unmodified crt_main.c and extra/video_convert.c linked against the libraries.
 
@@ -17,8 +17,7 @@ import numpy as np
 import pytest
 
 import support as S
-from ntsc_crt_b200 import capi, layout, sharding
-from sync_oracle import SYNC_VARIANTS, oracle_engine
+from ntsc_crt_b200 import capi, layout
 from test_simt_kernels import simt_libs  # noqa: F401  (session fixture of the interpreter builds)
 import test_simt_kernels as _simt
 
@@ -89,7 +88,7 @@ def check_batch(variant, generic=0, fields=8, big=(832, 624), small=(400, 300), 
         if layout.system_spec(variant).system == layout.SYS_VHS:
             m["seed"] = 100 + i
         mons.append(m)
-    rig = S.BatchRig(variant, mons, options=(("generic_eq", generic),), oracle=oracle_engine)
+    rig = S.BatchRig(variant, mons, options=(("generic_eq", generic),))
     imgs = [source(variant, 0, i)[0] for i in range(len(mons))]
     calls = [[] for _ in mons]  # per monitor and field: (poked (vsync, hsync) or None, settings, batch state after it)
     for it in range(fields):
@@ -137,7 +136,7 @@ def check_dropin(variant, outw=832, outh=624, fields=8):
     for it in range(fields):
         img, kw = source(variant, it, it % 2, seed=5)
         calls.append((POKES[it // 2 - 1] if it in (2, 4, 6) else None, img, kw, NOISES[it % 4] if it < 4 else (100, 255, 33, 60)[it % 4]))
-    gpu, ora = S.ProductEngine(variant, outw, outh), oracle_engine(variant, outw, outh)
+    gpu, ora = S.ProductEngine(variant, outw, outh), S.oracle_engine(variant, outw, outh)
     libc_srand(1)
     got = []
     for e in (gpu, ora):
@@ -173,7 +172,7 @@ def check_frames_host(variant, n=3, fields=4, outw=640, outh=480):
     if layout.system_spec(variant).system == layout.SYS_VHS:
         for i, m in enumerate(mons):
             m["seed"] = 7 + i
-    rig = S.BatchRig(variant, mons, oracle=oracle_engine)
+    rig = S.BatchRig(variant, mons)
     host = [torch.zeros(outh, outw, 4, dtype=torch.uint8).pin_memory() for _ in range(n)]
     srcs = []
     for i in range(n):
@@ -190,65 +189,18 @@ def check_frames_host(variant, n=3, fields=4, outw=640, outh=480):
         rig.check("%s frames_host field %d" % (variant, it))
         for i in range(n):
             got, want = host[i].numpy(), rig.oras[i].out
-            rows = np.zeros(outh, dtype=bool)
-            for l in rig.b.get_lines(i):
-                if l.beg >= 0:
-                    rows[l.beg:l.beg + max(1, l.end - 1 - l.beg)] = True
+            rows = S.written_rows(rig.b.get_lines(i), outh, 1)
             assert rows.any()
             assert np.array_equal(got[rows], want[rows]), (variant, it, i, S.diff_report("rows", got[rows], want[rows]))
     rig.close()
 
 
-def check_line_blocks(variant, world=2, outw=832, outh=624, fields=5):
-    """two contexts each decode their own block of lines (crtx_set_option line_lo / line_hi, sharding.ImageSharder);
-    the merged image equals the CPU model's sequential decode"""
-    import torch
-    noise = 60
-    ora = oracle_engine(variant, outw, outh)
-    ora.set(blend=1, scanlines=1)
-    ranks = []
-    for r in range(world):
-        b = capi.Batch(variant, 1)
-        if layout.system_spec(variant).system == layout.SYS_VHS:
-            b.seed(1, first=0, count=1)  # (the oracle's rand() replica is seeded with 1)
-        out = torch.zeros(outh, outw, 4, dtype=torch.uint8, device="cuda")
-        b.set_monitor(0, out, fmt=layout.PIX_BGRA, noise=noise, blend=1, scanlines=1)
-        b.commit_monitors()
-        part = sharding.ImageSharder(out, b.spec.lines, rank=r, world=world)
-        part.apply(b)
-        ranks.append((b, out, part))
-    for it in range(fields):
+def check_line_blocks(variant, outw=832, outh=624, fields=5):
+    """two contexts each decode their own block of lines (support.decode_in_blocks) at noise 60"""
+    def field(it):
         img, kw = source(variant, it, 1, seed=3)
-        dimg = torch.from_numpy(img.astype(np.int16) if img.dtype == np.uint16 else img).cuda()
-        if is_nes(variant):
-            ora.modulate(img, field_initialized=int(it != 0), **kw)
-        else:
-            ora.modulate(img, **kw)
-        ora.demodulate(noise)
-        ends = []
-        for r in range(world - 1):  # the halo rows ImageSharder.fetch_halo_rows hands over before the field
-            (_, dst, ps), (_, src, pn) = ranks[r], ranks[r + 1]
-            cnt = ps._halo_count(r)
-            if cnt:
-                dst[ps.r1:ps.r1 + cnt].copy_(src[pn.r0:pn.r0 + cnt])
-        for b, out, part in ranks:
-            b.set_source(0, dimg, **kw)
-            b.sources[0].reinit = int(it == 0)
-            b.modulate()
-            b.demodulate()
-            last = b.get_lines(0)[part.hi - 1]
-            ends.append(0 if last.beg < 0 else max(last.beg + 1, last.end - 1))
-        torch.cuda.synchronize()
-        for r in range(world - 1):  # the spill rows ImageSharder.exchange_spill_rows hands on after it
-            (_, src, ps), (_, dst, pd) = ranks[r], ranks[r + 1]
-            cnt = max(0, min(ends[r], outh, ps.r1 + ps.max_spill()) - ps.r1)
-            if cnt and pd.r0 == ps.r1:
-                dst[pd.r0:pd.r0 + cnt].copy_(src[ps.r1:ps.r1 + cnt])
-    full = np.zeros((outh, outw, 4), dtype=np.uint8)
-    for b, out, part in ranks:
-        full[part.r0:part.r1] = out[part.r0:part.r1].cpu().numpy()
-        b.close()
-    assert np.array_equal(full, ora.out), S.diff_report("merged image", full, ora.out)
+        return img, dict(kw, reinit=int(it == 0))
+    S.decode_in_blocks(variant, outw, outh, 2, field, fields=fields, noise=60)
 
 
 def check_video(noise=100, n=23, segments=5, outw=640, outh=480):
@@ -257,7 +209,7 @@ def check_video(noise=100, n=23, segments=5, outw=640, outh=480):
     import torch
     from ntsc_crt_b200 import video
     frames = S.moving_bars(n, 320, 240)
-    ora = oracle_engine("ntsc_nosync", outw, outh)
+    ora = S.oracle_engine("ntsc_nosync", outw, outh)
     ora.set(blend=0, scanlines=1, saturation=10)
     want = []
     for f in range(n):
@@ -275,25 +227,25 @@ def check_video(noise=100, n=23, segments=5, outw=640, outh=480):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("generic", [0, 1], ids=["fast_eq", "generic_eq"])
-@pytest.mark.parametrize("variant", SYNC_VARIANTS)
+@pytest.mark.parametrize("variant", capi.SYNC_VARIANTS)
 def test_batch_noise_geometries_and_poked_states(variant, generic):
     check_batch(variant, generic)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", SYNC_VARIANTS)
+@pytest.mark.parametrize("variant", capi.SYNC_VARIANTS)
 def test_dropin(variant):
     check_dropin(variant)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", SYNC_VARIANTS)
+@pytest.mark.parametrize("variant", capi.SYNC_VARIANTS)
 def test_frames_host(variant):
     check_frames_host(variant)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", SYNC_VARIANTS)
+@pytest.mark.parametrize("variant", capi.SYNC_VARIANTS)
 def test_line_blocks(variant):
     check_line_blocks(variant)
 
@@ -371,41 +323,18 @@ def test_unmodified_video_convert(tmp_path, flags, noise):
     shutil.rmtree(str(tmp_path / "b200"))
 
 
-@pytest.mark.parametrize("variant", SYNC_VARIANTS)
-def test_sync_library_exports_and_switches(variant):
-    """every symbol the headers declare is exported, and the library reports its system, timing and switches (capi.load
-    checks crtx_do_vsync / crtx_do_hsync against the variant too); every stock library reports both searches on"""
-    import test_capi_exports as X
-    lib = C.CDLL(capi.lib_path(variant))
-    for name in X.declared("crt_b200.h") + X.declared("crtx_batch.h"):
-        assert hasattr(lib, name), "%s missing from %s" % (name, variant)
-    lib = capi.load(variant)
-    spec = layout.system_spec(variant)
-    assert (lib.crtx_system(), lib.crtx_hres(), lib.crtx_do_vsync(), lib.crtx_do_hsync()) == (
-        spec.system, spec.hres, int(spec.do_vsync), int(spec.do_hsync))
-    assert not (spec.do_vsync and spec.do_hsync)
-    assert variant in capi.ALL_VARIANTS and variant not in capi.VARIANTS
-    for stock in capi.VARIANTS + capi.BORDER_VARIANTS:
-        s = capi.load(stock)
-        assert (s.crtx_do_vsync(), s.crtx_do_hsync()) == (1, 1), stock
-
-
 # ---- the same bodies on the CPU, through the SIMT interpreter ------------------------------------------------------
-# (the variants with a DEF_ line in csrc/Makefile, which tests/simt/build.py builds: all but vhs_nosync)
-INTERPRETED = [v for v in SYNC_VARIANTS if v in _simt.simt_build.variant_defines()]
-
-
 class TestOnTheInterpreter:
     simt_backend = staticmethod(_simt.simt_backend)  # autouse within this class: the interpreter builds, host "device" tensors
 
-    @pytest.mark.parametrize("variant", INTERPRETED)
+    @pytest.mark.parametrize("variant", capi.SYNC_VARIANTS)
     def test_batch(self, variant):
         check_batch(variant, fields=4, big=(528, 400), small=(320, 240), per_group=2)
 
     def test_batch_generic_eq(self):
         check_batch("ntsc_nosync", generic=1, fields=3, big=(528, 400), small=(320, 240), per_group=1)
 
-    @pytest.mark.parametrize("variant", INTERPRETED)
+    @pytest.mark.parametrize("variant", capi.SYNC_VARIANTS)
     def test_dropin(self, variant):
         check_dropin(variant, outw=320, outh=240, fields=4)
 

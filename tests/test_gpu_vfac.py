@@ -12,7 +12,6 @@ import pytest
 import support as S
 import test_oracle_vfac as V
 from ntsc_crt_b200 import layout
-from test_gpu_lineshard import decode_one_image_in_blocks
 from support import check, run_all, trio
 
 pytestmark = pytest.mark.gpu
@@ -141,9 +140,7 @@ def test_frames_host_rows_only_with_vfac(variant, monkeypatch):
             if not rows_only[i]:
                 assert np.array_equal(got, oras[i].out), "%s: %s" % (what, S.diff_report("host image", got, oras[i].out))
                 continue
-            for l in b.get_lines(i):
-                if l.beg >= 0:
-                    written[i][l.beg:l.beg + max(1, l.end - 1 - l.beg)] = True
+            written[i] |= S.written_rows(b.get_lines(i), outh, 1)
             w = written[i]
             assert 0 < w.sum() < outh or it > 0
             assert np.array_equal(got[w], oras[i].out[w]), "%s: %s" % (what, S.diff_report("written rows", got[w], oras[i].out[w]))
@@ -156,7 +153,7 @@ def test_frames_host_rows_only_with_vfac(variant, monkeypatch):
 def test_blocks_with_vfac(variant, outw, outh, v_fac, world):
     """the scanline-block partition with a stretching v_fac on an image shorter than the line count: the blocks'
     rows come from outh + v_fac (sharding.block_rows), lines past the image are skipped"""
-    decode_one_image_in_blocks(variant, outw, outh, 1, 1, world, v_fac=v_fac)
+    S.decode_in_blocks(variant, outw, outh, world, scanlines=1, blend=1, v_fac=v_fac)
 
 
 def test_launches_per_demodulate_by_span():

@@ -1,52 +1,31 @@
 """Pin the CPU model of the decoder with its sync searches off (tests/sync_oracle.py; CRT_DO_VSYNC 0 / CRT_DO_HSYNC 0,
 crt_core.h:71-72) against the reference compiled with the switches off (oracle/_ref/libref_<system>_<switches>.so, built
-by oracle/sync.mk): every system, each of the three switch sets, the whole state (analog, inp, out, ccf, hsync, vsync,
+by oracle/Makefile): every system, each of the three switch sets, the whole state (analog, inp, out, ccf, hsync, vsync,
 rn) after every call.  The fields span noise 0, 12, 60 and 255, interlaced and progressive sequences, vsync and hsync
 poked to far values through the struct, the knobs with v_fac, raw sources, and VHS with do_aberration.
 
-The reference builds' digests are recorded in tests/golden/sync_switches_ref.json.  Where oracle/_ref holds the builds
-they are run and must still give the recorded digests; elsewhere the records stand in for them.  SYNC_SWITCHES_RECORD=1
-rewrites the records of the tests it runs."""
+Where oracle/_ref holds the reference builds they are run; elsewhere their digests, recorded in
+tests/golden/ref_states.json (support.from_reference), stand in for them."""
 import hashlib
 import json
-import os
 
 import pytest
 
 import support as S
 from ntsc_crt_b200 import layout
-from sync_oracle import SWITCHES, SYSTEMS, oracle_engine
+from sync_oracle import SWITCHES, SYSTEMS
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "sync_switches_ref.json")
-RECORD = os.environ.get("SYNC_SWITCHES_RECORD") == "1"
 VARIANTS = ["%s_%s" % (s, w) for s in SYSTEMS for w in SWITCHES]
 
 
-def reference_digests(key, variant, run):
-    """run(make) on the reference build of `variant` where it exists, which must give the digests recorded under `key`
-    (SYNC_SWITCHES_RECORD=1 records them instead); else the recorded digests"""
-    path = S.ref_path(variant)
-    recs = json.load(open(GOLDEN)) if os.path.exists(GOLDEN) else {}
-    if not os.path.exists(path):
-        assert key in recs, "%s: no recorded reference digests in %s (oracle/_ref is not built here)" % (key, GOLDEN)
-        return recs[key]
-    got = run(lambda w, h, fmt: S.RefEngine(variant, w, h, fmt, seed=1))  # (VHS: libc rand() seeded as the oracle's)
-    if RECORD:
-        recs[key] = got
-        with open(GOLDEN, "w") as f:
-            f.write("{\n" + ",\n".join("%s: %s" % (json.dumps(k), json.dumps(recs[k])) for k in sorted(recs)) + "\n}\n")
-    else:
-        assert key in recs, "%s: no recorded reference digests in %s (record them with SYNC_SWITCHES_RECORD=1)" % (key, GOLDEN)
-        assert got == recs[key], "%s: the reference build no longer gives the digests recorded in %s" % (key, GOLDEN)
-    return got
-
-
-def check(key, variant, run):
-    want = reference_digests(key, variant, run)
-    got = run(lambda w, h, fmt: oracle_engine(variant, w, h, fmt))
-    assert len(got) == len(want), (key, len(got), len(want))
+def check(variant, run):
+    """run(make) with make(w, h, fmt) making the CPU model, against the same on the reference build of `variant` (VHS:
+    libc rand() seeded as the oracle's)"""
+    want = S.from_reference(S.ref_path(variant), lambda path: run(lambda w, h, fmt: S.RefEngine(variant, w, h, fmt, seed=1)))
+    got = run(lambda w, h, fmt: S.oracle_engine(variant, w, h, fmt))
+    assert len(got) == len(want), (len(got), len(want))
     bad = [i for i, (a, b) in enumerate(zip(got, want)) if a != b]
-    assert not bad, "%s: %d of %d states differ from the reference's, first after call %d" % (key, len(bad), len(want), bad[0])
+    assert not bad, "%d of %d states differ from the reference's, first after call %d" % (len(bad), len(want), bad[0])
 
 
 def state_hash(e):
@@ -93,7 +72,7 @@ def test_interlaced_with_noise_and_poked_sync(variant):
             e.demodulate([0, 12, 60, 255][it % 4])
             out.append(state_hash(e))
         return out
-    check("interlaced[%s]" % variant, variant, run)
+    check(variant, run)
 
 
 @pytest.mark.parametrize("variant", VARIANTS)
@@ -116,4 +95,4 @@ def test_progressive_knobs_vfac_raw(variant):
             e.demodulate([255, 60, 12, 0][it % 4])
             out.append(state_hash(e))
         return out
-    check("progressive[%s]" % variant, variant, run)
+    check(variant, run)

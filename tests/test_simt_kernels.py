@@ -242,7 +242,7 @@ def test_launch_count_is_the_kernels_launched(simt_libs, variant, monkeypatch):
         ran, counts = counted(one, lambda: (one.modulate(), one.demodulate()))
         assert ran == counts
         pair.append((dropin, counts))
-    assert pair[1][0] + (2 if variant == "vhs" else 0) == pair[1][1], pair
+    assert pair[1][0] + (2 if spec.system == layout.SYS_VHS else 0) == pair[1][1], pair
     one.close()
 
 
