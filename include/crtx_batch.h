@@ -99,7 +99,13 @@ int crtx_cc_vper(void);         /* CRT_CC_VPER */
 int  crtx_create(crtx_ctx **ctx, int n_monitors); /* on the current CUDA device */
 void crtx_destroy(crtx_ctx *ctx);
 
-/* configuration and state; `m` / `s` are HOST arrays of `count` entries */
+/* configuration and state; `m` / `s` are HOST arrays of `count` entries.
+ *
+ * crtx_set_monitors changes the host copy only: the next crtx_modulate / crtx_demodulate / crtx_frames_host, on
+ * whichever stream it is called, uploads every monitor changed since the last upload, then the calls on other streams
+ * wait for that upload.  A context may be driven from several streams over disjoint monitor ranges, but reconfigure a
+ * monitor only once the streams that have work queued for it are synchronised or waited on: the upload can otherwise
+ * overtake a decode still in flight on another stream. */
 int crtx_set_monitors(crtx_ctx *ctx, int first, int count, const crtx_monitor *m);
 int crtx_set_state(crtx_ctx *ctx, int first, int count, const crtx_state *s, void *stream);
 int crtx_get_state(crtx_ctx *ctx, int first, int count, crtx_state *s, void *stream);

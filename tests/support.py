@@ -306,9 +306,13 @@ class _ReplayRef:
 
     def __init__(self, variant, outw, outh, fmt=layout.PIX_BGRA, out=None, seed=None):
         self.spec = layout.system_spec(variant)
+        self.out = out
 
     def set(self, **kw):
         return self
+
+    def resize(self, outw, outh, fmt, out):
+        self.out = out
 
     def modulate(self, img, **kw):
         pass
@@ -631,6 +635,36 @@ def check(gpu, ora, ref, what):
         assert_same_state(gpu.state(), ref.state(), what + " [gpu vs reference]")
 
 
+def resize_sequence(variant, engines, check, fields=2):
+    """crt_resize between fields, on engines that start at 640 x 480 BGRA: `fields` fields, then as many after a
+    format-only resize (ARGB, the same image), after one to 333 x 250 RGB and after one to 832 x 624 BGRA (new zeroed
+    images).  The bytes behind inp[] (outw, outh, out_format of struct CRT) change with each.  check(what) after every
+    call."""
+    system = layout.system_spec(variant).system
+    steps = [None, (640, 480, layout.PIX_ARGB, False), (333, 250, layout.PIX_RGB, True), (832, 624, layout.PIX_BGRA, True)]
+    it = 0
+    for step in steps:
+        if step:
+            w, h, fmt, new = step
+            for e in engines:
+                e.resize(w, h, fmt, np.zeros((h, w, layout.bpp4fmt(fmt)), dtype=np.uint8) if new else e.out)
+        for _ in range(fields):
+            if system == layout.SYS_NES:
+                img, kw = nes_image(seed=it), dict(dot_crawl_offset=it % 3, hue=20 * it)
+            elif system == layout.SYS_NESRGB:
+                img, kw = rand_image(256, 240, seed=it), dict(format=layout.PIX_BGRA, dot_crawl_offset=it % 3)
+            else:
+                img, kw = rand_image(300, 220, seed=it), dict(format=layout.PIX_BGRA, as_color=1, field=it & 1, frame=0,
+                                                              dot_crawl_offset=it % 3)
+            for e in engines:
+                e.modulate(img, **kw)
+            check("%s after resize %s, field %d modulate" % (variant, step, it))
+            for e in engines:
+                e.demodulate(4 + it)
+            check("%s after resize %s, field %d demodulate" % (variant, step, it))
+            it += 1
+
+
 # ----------------------------------------------------------------------------------
 # the batch interface against one CPU model per monitor
 # ----------------------------------------------------------------------------------
@@ -646,30 +680,69 @@ def monitor_state(batch, i, out):
                 hsync=st.hsync, vsync=st.vsync, rn=st.rn)
 
 
+def struct_tail(batch, i):
+    """the 16 bytes behind monitor i's analog[] and inp[] on the device: what follows inp[] in the reference's struct CRT
+    (outw, outh, out_format, padding), which a decode window running past inp[] reads (k_struct_tail)"""
+    lib = batch.lib
+    lib.crtx_memcpy.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]
+    lib.crtx_sync.argtypes = [C.c_void_p]
+    tails = []
+    for ptr in (batch.analog_ptr(i), batch.inp_ptr(i)):
+        host = np.zeros(16, dtype=np.uint8)
+        batch._check(lib.crtx_memcpy(host.ctypes.data, ptr + batch.spec.input_size, 16, 1, None))
+        batch._check(lib.crtx_sync(None))
+        tails.append(host)
+    return tails
+
+
 class BatchRig:
     """A capi.Batch and one CPU model per monitor, driven through the same calls and compared whole state by whole state.
 
     mons[i] = dict(outw, outh, fmt, noise, knobs), and optionally seed: the VHS rand() seed of both sides.  options:
-    (name, value) pairs set on the batch first."""
+    (name, value) pairs set on the batch first.  outs: the monitors' output images where the caller makes them (windows of
+    larger tensors, say), zero-filled like the CPU models' images; None, or a None entry, for a dense image made here."""
 
-    def __init__(self, variant, mons, options=()):
-        import torch
+    def __init__(self, variant, mons, options=(), outs=None):
         from ntsc_crt_b200 import capi
         self.mons = mons
         self.b = capi.Batch(variant, len(mons))
         for name, value in options:
             self.b.set_option(name, value)
-        self.outs, self.oras, self._dev, self._src = [], [], {}, {}
+        self.outs, self.oras, self._dev, self._src = [None] * len(mons), [], {}, {}
         for i, m in enumerate(mons):
-            out = torch.zeros(m["outh"], m["outw"], max(1, layout.bpp4fmt(m["fmt"])), dtype=torch.uint8, device="cuda")
-            self.b.set_monitor(i, out, fmt=m["fmt"], noise=m["noise"], **m["knobs"])
+            self._monitor(i, m, outs[i] if outs else None)
             if "seed" in m:
                 self.b.seed(m["seed"], first=i, count=1)
             o = oracle_engine(variant, m["outw"], m["outh"], m["fmt"], seed=m.get("seed", 1))
             o.set(**m["knobs"])
-            self.outs.append(out)
             self.oras.append(o)
         self.b.commit_monitors()
+
+    def _monitor(self, i, m, out):
+        import torch
+        if out is None:
+            out = torch.zeros(m["outh"], m["outw"], max(1, layout.bpp4fmt(m["fmt"])), dtype=torch.uint8, device="cuda")
+        self.b.set_monitor(i, out, fmt=m["fmt"], noise=m["noise"], **m["knobs"])
+        self.outs[i] = out
+
+    def reconfigure(self, i, m, out=None):
+        """crtx_set_monitors on monitor i alone with the configuration m (knobs not in m["knobs"] back at crt_reset's), and
+        on its CPU model crt_resize + the knobs.  out: a new output image, zero-filled; None keeps the current one, which
+        must then still fit (outw, outh and the pixel size unchanged)."""
+        if out is None:
+            out = self.outs[i]
+            assert tuple(out.shape) == (m["outh"], m["outw"], max(1, layout.bpp4fmt(m["fmt"]))), (out.shape, m)
+            ora_out = self.oras[i].out
+        else:
+            ora_out = np.zeros(tuple(out.shape), dtype=np.uint8)
+        self._monitor(i, m, out)
+        self.b.commit_monitors(first=i, count=1)
+        knobs = dict(hue=0, brightness=0, contrast=180, saturation=10, black_point=0, white_point=100, scanlines=0, blend=0,
+                     v_fac=0)  # (Batch.set_monitor's defaults)
+        knobs.update(m["knobs"])
+        self.oras[i].resize(m["outw"], m["outh"], m["fmt"], ora_out)
+        self.oras[i].set(**knobs)
+        self.mons[i] = m
 
     def _device(self, img):
         import torch
@@ -713,8 +786,15 @@ class BatchRig:
         self.b.frames_host(host_ptrs)
 
     def check(self, what):
+        """every monitor's state against its CPU model's, and the bytes behind its signal buffers (struct_tail) against
+        its geometry"""
         for i, o in enumerate(self.oras):
             assert_same_state(monitor_state(self.b, i, self.outs[i]), o.state(), "%s, monitor %d %r" % (what, i, self.mons[i]))
+            m = self.mons[i]
+            want = np.array([m["outw"], m["outh"], m["fmt"], 0], dtype="<i4").view(np.uint8)
+            for which, got in zip(("analog", "inp"), struct_tail(self.b, i)):
+                assert np.array_equal(got, want), "%s, monitor %d %r: the 16 bytes behind %s[] are %r, not outw, outh, out_format, 0" % (
+                    what, i, m, which, got.view("<i4").tolist())
 
     def close(self):
         self.b.close()

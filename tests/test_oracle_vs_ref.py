@@ -365,6 +365,15 @@ def test_vhs(color, aberr):
         S.assert_same_state(a, b, "vhs demod %d" % it)
 
 
+@pytest.mark.parametrize("variant", ["ntsc", "vhs", "nes", "snes", "nesrgb", "template", "pv1k"])
+def test_resize_between_fields(variant):
+    """OracleEngine.resize is crt_resize (crt_core.c:241-248) between calls: a format-only change and size changes, on
+    every system, with the bytes behind inp[] that follow the geometry"""
+    ref, ora = pair(variant, 640, 480, seed=1)
+    both(ref, ora, lambda e: e.set(blend=1, scanlines=1))
+    S.resize_sequence(variant, (ref, ora), lambda what: check(ref, ora, what))
+
+
 def test_staged_decode_equals_whole_decode():
     """The oracle's three-stage split (what the kernels mirror) is the same function."""
     img = S.bars_image(400, 300)

@@ -19,6 +19,7 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "sim
 import build as simt_build  # noqa: E402
 
 import test_gpu_batch_api as _api  # noqa: E402
+import test_gpu_batch_fuzz as _bfuzz  # noqa: E402
 import test_gpu_bloom as _bloom  # noqa: E402
 import test_gpu_conv as _conv  # noqa: E402
 import test_gpu_dropin_cli as _cli  # noqa: E402
@@ -128,6 +129,50 @@ def small_vhs_runs(monkeypatch):
     monkeypatch.setattr(_vhs, "FIELDS", 3)
     monkeypatch.setattr(_vhs, "SWEEP_CASES", 1)
     monkeypatch.setattr(_vhs, "SWEEP_CALLS", 2)
+
+
+_BFUZZ_FULL = dict(MAX_MONITORS=_bfuzz.MAX_MONITORS, FIELDS=_bfuzz.FIELDS, MAX_OUTW=_bfuzz.MAX_OUTW)
+
+
+@pytest.fixture(autouse=True)
+def small_batch_sweeps(monkeypatch):
+    """tests/test_gpu_batch_fuzz.py with at most 4 monitors, 3 fields and outputs of 832 pixels or less; its streams are
+    stand-ins here (the interpreter runs every call in order, whatever the stream)"""
+    import contextlib
+    monkeypatch.setattr(_bfuzz, "MAX_MONITORS", 4)
+    monkeypatch.setattr(_bfuzz, "FIELDS", 3)
+    monkeypatch.setattr(_bfuzz, "MAX_OUTW", 832)
+    monkeypatch.setattr(_bfuzz, "make_streams", lambda k: [type("S", (), {"cuda_stream": 0})() for _ in range(k)])
+    monkeypatch.setattr(_bfuzz, "on_stream", lambda s: contextlib.nullcontext())
+
+
+# one draw each of a few systems (a whole draw of every variant costs minutes here); the coverage of the draws is the
+# GPU test's
+BFUZZ_CASES = [("ntsc", 1), ("ntsc", 2), ("pv1k", 1), ("nes", 1), ("nesrgb", 1), ("vhs", 1), ("ntsc_conv", 1), ("ntsc_bloom", 1),
+                ("nes_border", 1), ("ntsc_nosync", 1)]
+
+
+@pytest.mark.parametrize("variant,seed", BFUZZ_CASES, ids=["%s_seed%d" % c for c in BFUZZ_CASES])
+def test_bfuzz_random_batches(variant, seed):
+    _bfuzz.sweep(variant, seed)
+
+
+def test_bfuzz_full_size_draw(monkeypatch):
+    """one draw at the GPU test's sizes: ntsc seed 5 puts two monitors that differ in scanlines into one k_lines2 pair on
+    an image with more rows than lines, where scanlines changes the rows a line writes"""
+    for name, value in _BFUZZ_FULL.items():
+        monkeypatch.setattr(_bfuzz, name, value)
+    assert "lines2 pair differing in scanlines" in _bfuzz.sweep("ntsc", 5)
+
+
+@pytest.mark.parametrize("host", [0, 1])
+def test_bfuzz_streams(host, monkeypatch):
+    monkeypatch.setenv("SIMT_HOST_MAPPED", "1")  # (only the interpreter build of the library reads this)
+    _bfuzz.check_streams("ntsc", host, n_streams=2, fields=3)
+
+
+def test_bfuzz_dropin_resize():
+    _bfuzz.test_dropin_resize_between_fields("pv1k")
 
 
 def test_fullsize_property_on_a_small_batch(monkeypatch):
@@ -256,7 +301,7 @@ def test_other_thread_schedules(schedule):
     import subprocess
     env = dict(os.environ, SIMT_SCHEDULE=schedule)
     sel = ("(parity_batch_matches_the_oracle and not snes and not conv and not vhs) or wire_ppm or wire_fade or fullsize"
-           " or vfac_batch or vhs_batch_many_generator_states")
+           " or vfac_batch or vhs_batch_many_generator_states or (bfuzz_random_batches and ntsc_seed1)")
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-x", "-q", "-k", sel, "-p", "no:cacheprovider"],
                        env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, cwd=S.ROOT)
     assert r.returncode == 0, r.stdout[-3000:]
