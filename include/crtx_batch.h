@@ -116,7 +116,11 @@ signed char *crtx_analog(crtx_ctx *ctx, int i);
 signed char *crtx_inp(crtx_ctx *ctx, int i);
 
 /* copy monitor i's analog[] (which = 0) or inp[] (which = 1), CRT_INPUT_SIZE bytes, to / from a HOST
- * buffer; synchronises `stream` */
+ * buffer; synchronises `stream`.
+ * At noise 0 a demodulate does not write inp[] of the monitors its k_lines2 pass decodes: it equals analog[] with -128 read
+ * as -127, and it is made from analog[] when it is read here or when analog[] is written here.  A later crtx_modulate
+ * rewrites analog[]; reading such an inp[] after it fails and says so (crtx_last_error).  Once crtx_inp has handed out
+ * monitor i's pointer, every demodulate writes its inp[]. */
 int crtx_read_signal(crtx_ctx *ctx, int i, int which, signed char *host, void *stream);
 int crtx_write_signal(crtx_ctx *ctx, int i, int which, const signed char *host, void *stream);
 

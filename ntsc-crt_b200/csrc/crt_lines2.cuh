@@ -111,7 +111,8 @@ __device__ __forceinline__ void flush_tile(unsigned tile_q_a, unsigned old_a, Ti
 template <int MODE, int FMT> // MODE 0: no blend, 1: blend; FMT: one of the four 4-byte CRT_PIX_FORMATs
 __global__ void __launch_bounds__(kL2Threads, 1)
 k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, const LineRec *__restrict__ lines_base,
-         const signed char *__restrict__ inp_base, int first, int count, const LinesGeom geo)
+         const signed char *__restrict__ analog_base, const signed char *__restrict__ inp_base, int first, int count,
+         const LinesGeom geo)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -185,7 +186,12 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
     }
     const int rnd = geo.rnd;
 
-    const signed char *inp = inp_base + (size_t) m * kSignalBytes;
+    // the window source: analog[] where k_sync did not write inp[] (MonState::inp_late: noise 0, so inp[] would be
+    // max(analog[], -127): the clamp is applied to every sample below; k_sync leaves no window that reaches the struct tail
+    // behind the signal to this path), inp[] otherwise (no clamp: inp[] is clamped already and the tail is read raw)
+    const bool from_analog = states[m].inp_late != 0;
+    const signed char *inp = (from_analog ? analog_base : inp_base) + (size_t) m * kSignalBytes;
+    const int smin = from_analog ? -127 : -128;
     // stage c holds samples [c * kL2Stage, + kL2Stage) of the window: copied from the 16-byte aligned address at or
     // below its first sample (asynchronous copies move whole 16-byte words), found at byte (pos + c * kL2Stage) & 15
     const signed char *row_base = reinterpret_cast<const signed char *>(stage) + lane * kL2StageRow;
@@ -234,7 +240,7 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
             const unsigned yq_a = yiq_a + (sub & 1) * (kSub * 8);
 #pragma unroll
             for (int t = 0; t < kSub; t++) {
-                const int s = rp[t];
+                const int s = max((int) rp[t], smin); // (only moves -128, which analog[] may hold: a poked signal)
                 const int y = eq_step<kEqYlf, kEqYhf, kEqYg1, kEqYg2, true, true>(ey, s, rnd);
                 const int ci = eq_step<kEqIlf, kEqIhf, 65536, kEqIg2, true, false>(ei, wmul(s, wi[t % 4]) >> 9, rnd) >> 3;
                 const int cq = eq_step<kEqQlf, kEqQhf, 65536, 0, true, false>(eq, wmul(s, wq[t % 4]) >> 9, rnd) >> 3;

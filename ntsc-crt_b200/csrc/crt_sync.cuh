@@ -77,6 +77,7 @@ struct SyncShared {
     int generic;
     int noise_next; // next chunk of the noise pass to hand out (kFusedNoise)
     int need_max;   // some line of this pass needed its signal lines' largest sample
+    int need_inp;   // some line's window runs past inp[] into the struct tail, which must be read unclamped: inp[] after all
     int linemax[kVres + 2]; // largest |sample| of each signal line of inp[], measured by the noise pass when MonState::track_max says so
 };
 
@@ -190,10 +191,43 @@ __device__ __forceinline__ unsigned clamp127_4(unsigned x)
     return x | ((x & ~nz & 0x80808080u) >> 7);
 }
 
+// Vector t (16 samples) of inp[] at noise 0 from the same vector of analog[]: max(b, -127), and in the last vector only the
+// bytes inside inp[] (behind it lie the bytes of k_struct_tail, the same in both buffers)
+__device__ __forceinline__ void store_inp_vec(signed char *inp, int t, uint4 v)
+{
+    v.x = clamp127_4(v.x);
+    v.y = clamp127_4(v.y);
+    v.z = clamp127_4(v.z);
+    v.w = clamp127_4(v.w);
+    signed char *d = inp + t * kNoiseVec;
+    if ((t + 1) * kNoiseVec <= kInputSize) {
+        *reinterpret_cast<uint4 *>(d) = v;
+    } else {
+#pragma unroll
+        for (int b = 0; b < kNoiseVec; b++) {
+            const unsigned w = (b < 4) ? v.x : (b < 8) ? v.y : (b < 12) ? v.z : v.w;
+            if (t * kNoiseVec + b < kInputSize) d[b] = (signed char) (w >> (8 * (b & 3)));
+        }
+    }
+}
+
+// inp[] of the monitors whose last k_sync left it unwritten (MonState::inp_late), one CTA per monitor: what the host runs
+// before it hands inp[] out or lets analog[] change (crtx.cu: inp_from_analog)
+__global__ void __launch_bounds__(256) k_inp_from_analog(const MonState *__restrict__ states, const signed char *__restrict__ analog_base,
+                                                         signed char *__restrict__ inp_base, int first)
+{
+    const int m = first + blockIdx.x;
+    if (!states[m].inp_late) return;
+    const signed char *analog = analog_base + (size_t) m * kSignalBytes;
+    signed char *inp = inp_base + (size_t) m * kSignalBytes;
+    for (int t = threadIdx.x; t < kNoiseThreads; t += 256) store_inp_vec(inp, t, __ldg(reinterpret_cast<const uint4 *>(analog) + t));
+}
+
 // The LCG systems' noise pass is fused into this kernel (kFusedNoise): it reads analog[], applies the noise itself to what it
 // stages, and writes the whole inp[].  That copy is pure memory traffic and the burst-lock chain pure latency on one
 // warp, so they overlap: while the last warp runs the chain the other seven copy, 4 KB chunks handed out by a counter in shared
-// memory (the chain warp joins when it is through).
+// memory (the chain warp joins when it is through).  The overlap is not free: on the H100 the chain takes about 40 us beside
+// the copy and about 24 us without it (DESIGN.md, k_sync), so at noise 0 it is left out where it can be (inp_late).
 // VHS, whose noise comes from rand(): inp[] was written by k_noise_vhs, and this kernel reads it.
 constexpr bool kFusedNoise = !kIsVhs;
 constexpr int kNoiseNB = 8;                                   // 16-byte loads in flight per thread
@@ -240,9 +274,16 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
         return (int) (signed char) (w >> (8 * (p & 3)));
     };
     const int track = kFusedNoise ? st->track_max : 0; // measure every signal line's largest sample during the copy (see step 4)
+    // At noise 0 inp[] is max(analog[], -127).  For a monitor that k_lines2 decodes (MonCfg::lines2) the copy is not made:
+    // k_lines2 reads its windows from analog[] with that clamp, and the host produces inp[] when a caller asks for it
+    // (crtx.cu: inp_from_analog).  The copy would slow the burst-lock chain, which runs beside it on the same SM.  A monitor
+    // that turns out to need the generic equaliser (k_lines, which reads inp[]), or a window that reads the struct tail
+    // behind inp[] (bytes that may be -128 and are not clamped), gets it at the end after all.
+    bool inp_late = kFusedNoise && cfg.lines2 && noise == 0 && !track;
     if (tid == 0) {
         sh.noise_next = 0;
         sh.need_max = 0;
+        sh.need_inp = 0;
     }
     if (track)
         for (int l = tid; l < kVres + 2; l += kSyncThreads) sh.linemax[l] = 0;
@@ -544,7 +585,7 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
     }
     // ---- 3c. the noise pass proper (crt_core.c:346-367): analog -> inp, 16 samples per thread per round, 128-bit accesses,
     // by the seven warps that would otherwise wait for the chain (which joins them when it is through)
-    if (kFusedNoise) {
+    if (kFusedNoise && !inp_late) {
         for (;;) {
             int c = 0;
             if (lane == 0) c = atomicAdd(&sh.noise_next, 1);
@@ -708,6 +749,7 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
             // NES-RGB systems at their stock saturation, nothing else at stock settings), inside the copy that runs beside the
             // burst-lock chain; the first pass of such a monitor scans the two lines here instead, one thread per line, slowly.
             const int stail = (rec.pos + kAvLen > kInputSize) ? 128 : 0;
+            if (stail && inp_late) sh.need_inp = 1;
             int smax = max(127, stail);
             if (kFusedNoise && ((smax * wmax) >> 9) + 1 > 16383) {
                 sh.need_max = 1; // (the next pass of this monitor measures while it copies)
@@ -716,7 +758,8 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
                 } else {
                     const int lo = (g.ypos * kHres) & ~15, hi = min((g.ypos + 2) * kHres, kInputSize);
                     int mx = 0;
-                    for (int i = lo; i < hi; i++) mx = max(mx, abs((int) inp_w[i]));
+                    const signed char *sig = inp_late ? analog : inp_w; // (the clamp: inp[] not written yet)
+                    for (int i = lo; i < hi; i++) mx = max(mx, abs(max((int) sig[i], -127)));
                     smax = mx;
                 }
                 smax = max(smax, stail);
@@ -726,8 +769,13 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
         lines[k] = rec;
     }
     __syncthreads();
+    if (inp_late && (sh.generic || sh.need_inp)) {
+        for (int t = tid; t < kNoiseThreads; t += kSyncThreads) store_inp_vec(inp_w, t, __ldg(reinterpret_cast<const uint4 *>(analog) + t));
+        inp_late = false;
+    }
     if (tid == 0) {
         st->generic = sh.generic;
+        st->inp_late = inp_late;
         if (kFusedNoise) st->track_max = sh.need_max;
     }
     phase_mark(0, 14);

@@ -143,7 +143,7 @@ static void launch_lines2(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo
     with_mode4(geo.out_format, geo.blend, [&](auto mode, auto fmt) {
         constexpr int M = decltype(mode)::value, F = decltype(fmt)::value;
         k_lines2<M, F><<<(count + 1) / 2, kL2Threads, lines2_smem(geo.outw), stream>>>(ctx->d_cfg, ctx->d_state, ctx->d_lines,
-                                                                                         ctx->d_inp, lo, count, geo);
+                                                                                         ctx->d_analog, ctx->d_inp, lo, count, geo);
         ctx->launches += 1;
         ctx->lines2_launches += 1;
     });
@@ -322,6 +322,8 @@ int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cuda
 {
     if (check_range(ctx, first, count)) return 1;
     if (count == 0) return 0;
+    for (int i = first; i < first + count; i++)
+        if (ctx->h_inp_late[i] == 1) ctx->h_inp_late[i] = 2; // (the analog[] it would be made from is about to change)
     if (upload_cfg(ctx, stream)) return 1;
     CUDA_TRY(cudaMemcpyAsync(ctx->d_src + first, src, sizeof(SrcCfg) * count, cudaMemcpyHostToDevice, stream));
 #if (CRT_SYSTEM == CRT_SYSTEM_NTSCVHS)
@@ -412,11 +414,69 @@ static LinePasses line_passes(const MonCfg &c)
     return { 0, (int) ((kLines + run - 1) / run) + 1 };
 }
 
+// The line kernel takes the output geometry as launch-uniform arguments: a demodulate splits its range into runs of
+// monitors that share it (normally one run).  The row pitch is part of it: a batch of dense images, or of tiles of one
+// mosaic, has one pitch, so it costs no launch and the kernels read it from their parameters.  run_end: the end of the run
+// that starts at lo; run_geom: its geometry.
+static int run_end(const crtx_ctx *ctx, int lo, int end)
+{
+    const MonCfg &c0 = ctx->h_cfg[lo];
+    int hi = lo + 1;
+    while (hi < end) {
+        const MonCfg &c = ctx->h_cfg[hi];
+        if (c.outw != c0.outw || c.out_format != c0.out_format || c.blend != c0.blend || c.outh != c0.outh
+            || c.v_fac != c0.v_fac || c.out_pitch != c0.out_pitch)
+            break;
+        hi++;
+    }
+    return hi;
+}
+
+static LinesGeom run_geom(const crtx_ctx *ctx, int lo)
+{
+    const MonCfg &c0 = ctx->h_cfg[lo];
+    LinesGeom geo;
+    geo.outw = c0.outw;
+    geo.out_format = c0.out_format;
+    geo.bpp = c0.bpp;
+    geo.pitch = c0.out_pitch;
+    geo.blend = c0.blend ? 1 : 0;
+    geo.rnd = 32768;
+    geo.dx = c0.outw > 0 ? ((kAvLen - 1) << 12) / c0.outw : 0;
+    geo.line_lo = ctx->opt_line_lo;
+    geo.line_hi = ctx->opt_line_hi;
+    geo.pass = line_passes(c0).first;
+    return geo;
+}
+
+// MonCfg::lines2 of every monitor in [first, first + count): whether this demodulate's line pass is k_lines2, which then
+// decodes from analog[] where k_sync leaves inp[] unwritten (crt_sync.cuh: inp_late), and no raw pointer to the monitor's
+// inp[] was handed out.  A change travels with the next upload_cfg.
+static void mark_lines2(crtx_ctx *ctx, int first, int count)
+{
+    for (int lo = first; lo < first + count;) {
+        const int hi = run_end(ctx, lo, first + count);
+        const LinesGeom geo = run_geom(ctx, lo);
+        const bool eligible = lines2_eligible(ctx, hi - lo, lo, geo);
+        for (int i = lo; i < hi; i++) {
+            const int want = (eligible && !ctx->h_inp_pinned[i]) ? 1 : 0;
+            if (ctx->h_cfg[i].lines2 == want) continue;
+            ctx->h_cfg[i].lines2 = want;
+            if (i < ctx->cfg_dirty_lo) ctx->cfg_dirty_lo = i;
+            if (i + 1 > ctx->cfg_dirty_hi) ctx->cfg_dirty_hi = i + 1;
+        }
+        lo = hi;
+    }
+}
+
 int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, const short *d_noise_terms)
 {
     if (check_range(ctx, first, count)) return 1;
     if (count == 0) return 0;
+    mark_lines2(ctx, first, count);
     if (upload_cfg(ctx, stream)) return 1;
+    for (int i = first; i < first + count; i++)
+        ctx->h_inp_late[i] = (kFusedNoise && ctx->h_cfg[i].lines2 && ctx->h_cfg[i].noise == 0) ? 1 : 0;
 #if (CRT_SYSTEM == CRT_SYSTEM_NTSCVHS)
     if (d_noise_terms) { // drop-in path: the terms were drawn from the process's libc on the host
         dim3 tgrid((kInputSize + 255) / 256, count);
@@ -450,31 +510,11 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
         k_bloom<<<count, 256, 0, stream>>>(ctx->d_cfg, ctx->d_lines, ctx->d_inp, static_cast<BloomLine *>(ctx->d_bloom), first);
         ctx->launches += 1;
     }
-    // The line kernel takes the output geometry as launch-uniform arguments: split the range into
-    // runs of monitors that share it (normally one run).  The row pitch is part of it: a batch of dense images, or of
-    // tiles of one mosaic, has one pitch, so it costs no launch and the kernels read it from their parameters.
     for (int lo = first; lo < first + count;) {
-        const MonCfg &c0 = ctx->h_cfg[lo];
-        int hi = lo + 1;
-        while (hi < first + count) {
-            const MonCfg &c = ctx->h_cfg[hi];
-            if (c.outw != c0.outw || c.out_format != c0.out_format || c.blend != c0.blend || c.outh != c0.outh
-                || c.v_fac != c0.v_fac || c.out_pitch != c0.out_pitch)
-                break;
-            hi++;
-        }
-        LinesGeom geo;
-        geo.outw = c0.outw;
-        geo.out_format = c0.out_format;
-        geo.bpp = c0.bpp;
-        geo.pitch = c0.out_pitch;
-        geo.blend = c0.blend ? 1 : 0;
-        geo.rnd = 32768;
-        geo.dx = c0.outw > 0 ? ((kAvLen - 1) << 12) / c0.outw : 0;
-        geo.line_lo = ctx->opt_line_lo;
-        geo.line_hi = ctx->opt_line_hi;
+        const int hi = run_end(ctx, lo, first + count);
+        LinesGeom geo = run_geom(ctx, lo);
         LaunchTimer lt(ctx, stream, 4);
-        const LinePasses passes = line_passes(c0);
+        const LinePasses passes = line_passes(ctx->h_cfg[lo]);
         for (int p = 0; p < passes.count; p++) {
             geo.pass = passes.first + p;
             launch_lines(ctx, hi - lo, lo, geo, stream);
@@ -482,6 +522,26 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
         lo = hi;
     }
     CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int inp_from_analog(crtx_ctx *ctx, int first, int count, cudaStream_t stream)
+{
+    // one launch per run of monitors marked 1: a monitor outside them may carry a stale device flag, and its analog[] may
+    // have changed since
+    for (int lo = first; lo < first + count;) {
+        if (ctx->h_inp_late[lo] != 1) {
+            lo++;
+            continue;
+        }
+        int hi = lo + 1;
+        while (hi < first + count && ctx->h_inp_late[hi] == 1) hi++;
+        k_inp_from_analog<<<hi - lo, 256, 0, stream>>>(ctx->d_state, ctx->d_analog, ctx->d_inp, lo);
+        ctx->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+        for (int i = lo; i < hi; i++) ctx->h_inp_late[i] = 0;
+        lo = hi;
+    }
     return 0;
 }
 
@@ -761,6 +821,8 @@ int crtx_create(crtx_ctx **out, int n)
     ctx->h_cfg.assign(n, MonCfg());
     memset(ctx->h_cfg.data(), 0, sizeof(MonCfg) * n);
     ctx->h_mod_staged.assign(n, 0);
+    ctx->h_inp_late.assign(n, 0);
+    ctx->h_inp_pinned.assign(n, 0);
     ctx->cfg_dirty_lo = 0;
     ctx->cfg_dirty_hi = n;
     ctx->tail_dirty_lo = 0;
@@ -905,6 +967,7 @@ int crtx_set_monitors(crtx_ctx *ctx, int first, int count, const crtx_monitor *m
         c.noise = m[i].noise;
         c.out_pitch = m[i].out_pitch ? m[i].out_pitch : c.outw * c.bpp;
         MonCfg &old = ctx->h_cfg[first + i];
+        c.lines2 = old.lines2; // (the demodulate's to set)
         if (memcmp(&c, &old, sizeof(MonCfg)) == 0) continue;
         if (c.outw != old.outw || c.outh != old.outh || c.out_format != old.out_format) {
             if (first + i < tlo) tlo = first + i;
@@ -984,9 +1047,18 @@ signed char *crtx_analog(crtx_ctx *ctx, int i)
     return ctx->d_analog + (size_t) i * kSignalBytes;
 }
 
+// The caller may read or write inp[] through the pointer at any time: from now on k_sync writes it on every demodulate
+// (mark_lines2), and what the last demodulate left unwritten is made now, after the work already queued on any stream.
 signed char *crtx_inp(crtx_ctx *ctx, int i)
 {
     if (check_range(ctx, i, 1)) return NULL;
+    ctx->h_inp_pinned[i] = 1;
+    if (ctx->h_inp_late[i] == 1) {
+        if (cudaDeviceSynchronize() != cudaSuccess || inp_from_analog(ctx, i, 1, 0) || cudaDeviceSynchronize() != cudaSuccess) {
+            fail("crtx_inp: making monitor %d's inp[] failed", i);
+            return NULL;
+        }
+    }
     return ctx->d_inp + (size_t) i * kSignalBytes;
 }
 
@@ -994,6 +1066,10 @@ int crtx_read_signal(crtx_ctx *ctx, int i, int which, signed char *host, void *s
 {
     if (check_range(ctx, i, 1)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (which && ctx->h_inp_late[i] == 2)
+        return fail("monitor %d: inp[] of the last demodulate was decoded from analog[] (noise 0) and not kept, and a modulate has "
+                    "rewritten analog[] since; crtx_inp(ctx, %d) keeps it from the next demodulate on", i, i);
+    if (which && inp_from_analog(ctx, i, 1, st)) return 1;
     const signed char *src = (which ? ctx->d_inp : ctx->d_analog) + (size_t) i * kSignalBytes;
     CUDA_TRY(cudaMemcpyAsync(host, src, kInputSize, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -1004,6 +1080,8 @@ int crtx_write_signal(crtx_ctx *ctx, int i, int which, const signed char *host, 
 {
     if (check_range(ctx, i, 1)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (which) ctx->h_inp_late[i] = 0;                          // (the caller's inp[] replaces it)
+    else if (inp_from_analog(ctx, i, 1, st)) return 1;           // (before the analog[] it is made from changes)
     signed char *dst = (which ? ctx->d_inp : ctx->d_analog) + (size_t) i * kSignalBytes;
     CUDA_TRY(cudaMemcpyAsync(dst, host, kInputSize, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaStreamSynchronize(st));

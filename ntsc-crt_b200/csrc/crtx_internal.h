@@ -38,6 +38,10 @@ struct crtx_ctx {
     std::vector<crt::MonCfg> h_cfg;
     std::vector<unsigned char> h_mod_staged; // per monitor: the last modulate encoded its picture with k_mod_picture_rgb_staged (crtx_get_paths)
     std::vector<crt::SrcCfg> scratch_src;
+    // per monitor, inp[] at noise 0 (crt_sync.cuh: inp_late): 1 = the last demodulate may have left it unwritten, to be made
+    // from analog[] when it is handed out; 2 = ... and a modulate has rewritten analog[] since, so it is gone
+    std::vector<unsigned char> h_inp_late;
+    std::vector<unsigned char> h_inp_pinned; // crtx_inp handed out a raw pointer: k_sync writes inp[] on every demodulate
     int cfg_dirty_lo = 0, cfg_dirty_hi = 0;
     int tail_dirty_lo = 0, tail_dirty_hi = 0; // monitors whose output geometry changed: k_struct_tail rewrites the bytes behind their signals
     cudaEvent_t cfg_ready = nullptr;   // recorded behind the last configuration upload; launches on other streams wait on it
@@ -67,4 +71,6 @@ void fill_src(SrcCfg *d, const crtx_source *s);
 int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cudaStream_t stream);
 // d_noise_terms: VHS only -- per-sample noise term already drawn on the host from libc rand()
 int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, const short *d_noise_terms);
+// inp[] of monitors [first, first + count) made from analog[] where the last demodulate left it (ordered on `stream`)
+int inp_from_analog(crtx_ctx *ctx, int first, int count, cudaStream_t stream);
 } // namespace crt
