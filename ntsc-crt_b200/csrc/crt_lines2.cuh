@@ -188,7 +188,8 @@ k_lines2(const MonCfg *__restrict__ cfgs, const MonState *__restrict__ states, c
 
     // the window source: analog[] where k_sync did not write inp[] (MonState::inp_late: noise 0, so inp[] would be
     // max(analog[], -127): the clamp is applied to every sample below; k_sync leaves no window that reaches the struct tail
-    // behind the signal to this path), inp[] otherwise (no clamp: inp[] is clamped already and the tail is read raw)
+    // behind the signal to this path), inp[] otherwise (no clamp: inp[] is clamped already and the tail is read raw).
+    // Either way inp[] is only read here; the host makes a late one from analog[] (crtx.cu: inp_from_analog).
     const bool from_analog = states[m].inp_late != 0;
     const signed char *inp = (from_analog ? analog_base : inp_base) + (size_t) m * kSignalBytes;
     const int smin = from_analog ? -127 : -128;

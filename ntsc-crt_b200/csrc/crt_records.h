@@ -18,7 +18,7 @@ struct MonCfg { // host -> device, the caller-settable part of struct CRT
     unsigned v_fac;
     int noise;
     int out_pitch; // bytes between output rows (never 0: the host resolves crtx_monitor's 0 to outw * bpp)
-    int lines2;    // host-managed: k_lines2 decodes this monitor, so at noise 0 it can write inp[] in k_sync's place (crtx.cu)
+    int lines2;    // host-managed: k_lines2 decodes this monitor, so at noise 0 k_sync may leave inp[] unwritten (crtx.cu)
 };
 
 struct MonState { // device resident, the persistent decoder state of struct CRT
@@ -28,7 +28,7 @@ struct MonState { // device resident, the persistent decoder state of struct CRT
     int generic; // last sync pass: some line needs the wrap-exact (generic) equaliser path
     int track_max; // last sync pass: some line's carrier was large enough for the fast path to hinge on the line's largest sample:
                    // the next pass measures every signal line's while it copies it (crt_sync.cuh); device-managed
-    int inp_late;  // last sync pass left inp[] to k_lines2, which decodes from analog[] and writes inp[] as it goes
+    int inp_late;  // last sync pass left inp[] unwritten: k_lines2 decodes from analog[], clamping each sample as it reads it
 };
 
 struct SrcCfg { // host -> device, struct NTSC_SETTINGS

@@ -131,31 +131,67 @@ __global__ void __launch_bounds__(64) k_struct_tail(const MonCfg *__restrict__ c
     }
 }
 
-// Four samples of inp[] starting at the 4-aligned index p, computed from the word `w` of analog[] exactly
-// as the noise pass does (crt_core.c:346-367): sample i uses the LCG state advanced i + 1 steps from the
-// call's seed.  Kept apart from the load so that callers can issue a batch of loads before touching any.
+// max(b, -127) on four packed samples (the clamp of crt_core.c:363-364 when the noise term is zero: only -128 moves).
+// A byte is 0x80 iff its top bit is set and its low seven bits are zero; (low7 + 0x7f) carries into the top bit iff they are not.
+__device__ __forceinline__ unsigned clamp127_4(unsigned x)
+{
+    const unsigned nz = (x & 0x7f7f7f7fu) + 0x7f7f7f7fu;
+    return x | ((x & ~nz & 0x80808080u) >> 7);
+}
+__device__ __forceinline__ uint4 clamp127_v(uint4 v)
+{
+    return make_uint4(clamp127_4(v.x), clamp127_4(v.y), clamp127_4(v.z), clamp127_4(v.w));
+}
+
+// The noise pass (crt_core.c:346-367) at noise != 0: sample i of inp[] is analog[i] plus the noise term of the LCG state
+// advanced i + 1 steps from the call's seed rn0, clamped to +-127.  noise_state: the state before sample 16 t, from the
+// jump tables; noise_word: four samples from the state before them, which it advances past them.
+__device__ __forceinline__ unsigned noise_state(int t, unsigned rn0, const Affine *__restrict__ jump_lo, const Affine *__restrict__ jump_hi)
+{
+    const Affine lo = jump_lo[t % kJumpLo], hi = jump_hi[t / kJumpLo];
+    return (rn0 * hi.mul + hi.add) * lo.mul + lo.add;
+}
+__device__ __forceinline__ unsigned noise_word(unsigned w, unsigned &rn, int noise)
+{
+    unsigned o = 0;
+#pragma unroll
+    for (int b = 0; b < 4; b++) {
+        rn = rn * kLcgMul + kLcgAdd;
+        const int v = (int) (signed char) (w >> (8 * b)) + (wmul((int) ((rn >> 16) & 0xff) - 0x7f, noise) >> 8);
+        o |= ((unsigned) clampi(v, -127, 127) & 0xffu) << (8 * b);
+    }
+    return o;
+}
+
+// Vector t of inp[] (samples 16 t .. 16 t + 15) from the same 16 bytes of analog[].  Its bytes past inp[] (the last vector
+// runs over) are noised like the rest: its callers store and measure only the bytes inside.
+__device__ __forceinline__ uint4 noisy_vec(uint4 v, int t, int noise, unsigned rn0, const Affine *__restrict__ jump_lo,
+                                           const Affine *__restrict__ jump_hi)
+{
+    if (noise == 0) return clamp127_v(v);
+    unsigned rn = noise_state(t, rn0, jump_lo, jump_hi);
+    v.x = noise_word(v.x, rn, noise);
+    v.y = noise_word(v.y, rn, noise);
+    v.z = noise_word(v.z, rn, noise);
+    v.w = noise_word(v.w, rn, noise);
+    return v;
+}
+
+// The same rule for the four samples starting at the 4-aligned index p, from the word `w` of analog[] there, for what k_sync
+// stages and reads.  Beyond inp[] lie the bytes k_struct_tail put there (what follows inp[] inside the reference's struct
+// CRT), identical after analog[] and after inp[], and never touched by the noise pass: they are kept raw.  Kept apart from
+// the load so that callers can issue a batch of loads before touching any.
 __device__ __forceinline__ unsigned noisy_apply(unsigned w, int p, int noise, unsigned rn0,
                                                 const Affine *__restrict__ jump_lo, const Affine *__restrict__ jump_hi)
 {
     const unsigned raw = w;
     if (noise == 0) {
-        w = __vmaxs4(w, 0x81818181u);
+        w = clamp127_4(w);
     } else {
-        const int t = p / kNoiseVec;
-        const Affine lo = jump_lo[t % kJumpLo], hi = jump_hi[t / kJumpLo];
-        unsigned rn = (rn0 * hi.mul + hi.add) * lo.mul + lo.add; // state before sample 16 t
+        unsigned rn = noise_state(p / kNoiseVec, rn0, jump_lo, jump_hi);
         for (int k = 0; k < (p % kNoiseVec); k++) rn = rn * kLcgMul + kLcgAdd;
-        unsigned o = 0;
-#pragma unroll
-        for (int b = 0; b < 4; b++) {
-            rn = rn * kLcgMul + kLcgAdd;
-            int v = (int) (signed char) (w >> (8 * b)) + (wmul((int) ((rn >> 16) & 0xff) - 0x7f, noise) >> 8);
-            o |= ((unsigned) clampi(v, -127, 127) & 0xffu) << (8 * b);
-        }
-        w = o;
+        w = noise_word(w, rn, noise);
     }
-    // beyond inp[] lie the bytes k_struct_tail put there (what follows inp[] inside the reference's struct CRT),
-    // identical after analog[] and after inp[], and never touched by the noise pass: keep them raw
     if (p + 4 > kInputSize) {
         const unsigned keep = (p >= kInputSize) ? 0u : (0xffffffffu >> (8 * (p + 4 - kInputSize))); // bytes still inside inp[]
         w = (w & keep) | (raw & ~keep);
@@ -183,22 +219,10 @@ __device__ __forceinline__ unsigned max127_4(unsigned a, unsigned b)
     return (a & sel) | (b & ~sel);
 }
 
-// max(b, -127) on four packed samples (the clamp of crt_core.c:363-364 when the noise term is zero: only -128 moves).
-// A byte is 0x80 iff its top bit is set and its low seven bits are zero; (low7 + 0x7f) carries into the top bit iff they are not.
-__device__ __forceinline__ unsigned clamp127_4(unsigned x)
-{
-    const unsigned nz = (x & 0x7f7f7f7fu) + 0x7f7f7f7fu;
-    return x | ((x & ~nz & 0x80808080u) >> 7);
-}
-
-// Vector t (16 samples) of inp[] at noise 0 from the same vector of analog[]: max(b, -127), and in the last vector only the
-// bytes inside inp[] (behind it lie the bytes of k_struct_tail, the same in both buffers)
+// Writes vector t of inp[] (noisy_vec's result): in the last vector only the bytes inside inp[] (behind it lie the bytes of
+// k_struct_tail, the same in both buffers)
 __device__ __forceinline__ void store_inp_vec(signed char *inp, int t, uint4 v)
 {
-    v.x = clamp127_4(v.x);
-    v.y = clamp127_4(v.y);
-    v.z = clamp127_4(v.z);
-    v.w = clamp127_4(v.w);
     signed char *d = inp + t * kNoiseVec;
     if ((t + 1) * kNoiseVec <= kInputSize) {
         *reinterpret_cast<uint4 *>(d) = v;
@@ -220,7 +244,7 @@ __global__ void __launch_bounds__(256) k_inp_from_analog(const MonState *__restr
     if (!states[m].inp_late) return;
     const signed char *analog = analog_base + (size_t) m * kSignalBytes;
     signed char *inp = inp_base + (size_t) m * kSignalBytes;
-    for (int t = threadIdx.x; t < kNoiseThreads; t += 256) store_inp_vec(inp, t, __ldg(reinterpret_cast<const uint4 *>(analog) + t));
+    for (int t = threadIdx.x; t < kNoiseThreads; t += 256) store_inp_vec(inp, t, clamp127_v(__ldg(reinterpret_cast<const uint4 *>(analog) + t)));
 }
 
 // The LCG systems' noise pass is fused into this kernel (kFusedNoise): it reads analog[], applies the noise itself to what it
@@ -340,8 +364,11 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
             unsigned w[4] = { v[b].x, v[b].y, v[b].z, v[b].w };
             if (kFusedNoise && pos >= 0 && !raw_cand(b * kSyncThreads + tid)) {
                 if (noise == 0 && pos + 16 <= kInputSize) {
-#pragma unroll
-                    for (int e = 0; e < 4; e++) w[e] = clamp127_4(w[e]);
+                    const uint4 c = clamp127_v(v[b]);
+                    w[0] = c.x;
+                    w[1] = c.y;
+                    w[2] = c.z;
+                    w[3] = c.w;
                 } else {
 #pragma unroll 1
                     for (int e = 0; e < 4; e++) w[e] = noisy_apply(w[e], pos + 4 * e, noise, rn0, jump_lo, jump_hi);
@@ -593,13 +620,22 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
             if (c >= kNoiseChunks) break;
             const int t0 = c * kNoiseChunkVecs + lane;
             // largest |sample| of the vector's 16 bytes (already clamped to +-127), credited to the signal line(s) they lie in
-            auto track_vec = [&](unsigned w0, unsigned w1, unsigned w2, unsigned w3, int i0) {
-                unsigned a = max127_4(max127_4(abs127_4(w0), abs127_4(w1)), max127_4(abs127_4(w2), abs127_4(w3)));
+            auto track_vec = [&](uint4 v, int i0) {
+                unsigned a = max127_4(max127_4(abs127_4(v.x), abs127_4(v.y)), max127_4(abs127_4(v.z), abs127_4(v.w)));
                 a = max127_4(a, a >> 16);
                 const int mx = (int) (max127_4(a, a >> 8) & 0xffu);
                 const int l0 = i0 / kHres, l1 = min(i0 + kNoiseVec - 1, kInputSize - 1) / kHres;
                 if (mx > sh.linemax[l0]) atomicMax(&sh.linemax[l0], mx);
                 if (l1 != l0 && mx > sh.linemax[l1]) atomicMax(&sh.linemax[l1], mx);
+            };
+            auto inside_inp = [&](uint4 v, int i0) { // the vector's bytes inside inp[], 0 behind it (not signal)
+                unsigned w[4] = { v.x, v.y, v.z, v.w };
+#pragma unroll
+                for (int e = 0; e < 4; e++) {
+                    const int left = kInputSize - i0 - 4 * e; // bytes of word e inside inp[]
+                    w[e] = (left <= 0) ? 0u : (left >= 4) ? w[e] : (w[e] & (0xffffffffu >> (8 * (4 - left))));
+                }
+                return make_uint4(w[0], w[1], w[2], w[3]);
             };
             if (noise == 0 && (c + 1) * kNoiseChunkVecs * kNoiseVec <= kInputSize) { // whole vectors, no noise term: the stock case
                 uint4 in[kNoiseNB];
@@ -607,15 +643,13 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
                 for (int u = 0; u < kNoiseNB; u++) in[u] = *reinterpret_cast<const uint4 *>(analog + (t0 + 32 * u) * kNoiseVec);
 #pragma unroll
                 for (int u = 0; u < kNoiseNB; u++) {
-                    in[u].x = clamp127_4(in[u].x);
-                    in[u].y = clamp127_4(in[u].y);
-                    in[u].z = clamp127_4(in[u].z);
-                    in[u].w = clamp127_4(in[u].w);
-                    *reinterpret_cast<uint4 *>(inp_w + (t0 + 32 * u) * kNoiseVec) = in[u];
+                    if ((t0 + 32 * u + 1) * kNoiseVec > kInputSize) __builtin_unreachable(); // (a whole chunk: no partial vector)
+                    in[u] = clamp127_v(in[u]);
+                    store_inp_vec(inp_w, t0 + 32 * u, in[u]);
                 }
                 if (track) {
 #pragma unroll
-                    for (int u = 0; u < kNoiseNB; u++) track_vec(in[u].x, in[u].y, in[u].z, in[u].w, (t0 + 32 * u) * kNoiseVec);
+                    for (int u = 0; u < kNoiseNB; u++) track_vec(in[u], (t0 + 32 * u) * kNoiseVec);
                 }
                 continue;
             }
@@ -624,37 +658,9 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
                 const int t = t0 + 32 * u;
                 if (t >= kNoiseThreads) continue;
                 const int i0 = t * kNoiseVec;
-                const uint4 in = *reinterpret_cast<const uint4 *>(analog + i0);
-                unsigned w[4] = { in.x, in.y, in.z, in.w };
-                if (noise == 0) {
-#pragma unroll
-                    for (int e = 0; e < 4; e++) w[e] = clamp127_4(w[e]);
-                } else {
-                    const Affine lo = jump_lo[t % kJumpLo], hi = jump_hi[t / kJumpLo];
-                    unsigned rn = (rn0 * hi.mul + hi.add) * lo.mul + lo.add;
-#pragma unroll
-                    for (int e = 0; e < 4; e++) {
-                        unsigned o = 0;
-#pragma unroll
-                        for (int b = 0; b < 4; b++) {
-                            rn = rn * kLcgMul + kLcgAdd;
-                            int v = (int) (signed char) (w[e] >> (8 * b)) + (wmul((int) ((rn >> 16) & 0xff) - 0x7f, noise) >> 8);
-                            o |= ((unsigned) clampi(v, -127, 127) & 0xffu) << (8 * b);
-                        }
-                        w[e] = o;
-                    }
-                }
-                if (i0 + kNoiseVec <= kInputSize) {
-                    *reinterpret_cast<uint4 *>(inp_w + i0) = make_uint4(w[0], w[1], w[2], w[3]);
-                } else {
-                    for (int b = 0; i0 + b < kInputSize; b++) inp_w[i0 + b] = (signed char) (w[b >> 2] >> (8 * (b & 3)));
-#pragma unroll
-                    for (int e = 0; e < 4; e++) { // (what lies behind inp[] is not signal)
-                        const int left = kInputSize - i0 - 4 * e; // bytes of word e inside inp[]
-                        w[e] = (left <= 0) ? 0u : (left >= 4) ? w[e] : (w[e] & (0xffffffffu >> (8 * (4 - left))));
-                    }
-                }
-                if (track) track_vec(w[0], w[1], w[2], w[3], i0);
+                uint4 v = noisy_vec(*reinterpret_cast<const uint4 *>(analog + i0), t, noise, rn0, jump_lo, jump_hi);
+                store_inp_vec(inp_w, t, v);
+                if (track) track_vec(i0 + kNoiseVec <= kInputSize ? v : inside_inp(v, i0), i0);
             }
         }
         phase_mark(0, 7);
@@ -770,7 +776,7 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
     }
     __syncthreads();
     if (inp_late && (sh.generic || sh.need_inp)) {
-        for (int t = tid; t < kNoiseThreads; t += kSyncThreads) store_inp_vec(inp_w, t, __ldg(reinterpret_cast<const uint4 *>(analog) + t));
+        for (int t = tid; t < kNoiseThreads; t += kSyncThreads) store_inp_vec(inp_w, t, clamp127_v(__ldg(reinterpret_cast<const uint4 *>(analog) + t)));
         inp_late = false;
     }
     if (tid == 0) {

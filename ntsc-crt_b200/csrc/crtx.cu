@@ -323,7 +323,7 @@ int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cuda
     if (check_range(ctx, first, count)) return 1;
     if (count == 0) return 0;
     for (int i = first; i < first + count; i++)
-        if (ctx->h_inp_late[i] == 1) ctx->h_inp_late[i] = 2; // (the analog[] it would be made from is about to change)
+        if (ctx->h_inp[i] == kInpLate) ctx->h_inp[i] = kInpGone; // (the analog[] it would be made from is about to change)
     if (upload_cfg(ctx, stream)) return 1;
     CUDA_TRY(cudaMemcpyAsync(ctx->d_src + first, src, sizeof(SrcCfg) * count, cudaMemcpyHostToDevice, stream));
 #if (CRT_SYSTEM == CRT_SYSTEM_NTSCVHS)
@@ -459,7 +459,7 @@ static void mark_lines2(crtx_ctx *ctx, int first, int count)
         const LinesGeom geo = run_geom(ctx, lo);
         const bool eligible = lines2_eligible(ctx, hi - lo, lo, geo);
         for (int i = lo; i < hi; i++) {
-            const int want = (eligible && !ctx->h_inp_pinned[i]) ? 1 : 0;
+            const int want = (eligible && !inp_pinned(ctx->h_inp[i])) ? 1 : 0;
             if (ctx->h_cfg[i].lines2 == want) continue;
             ctx->h_cfg[i].lines2 = want;
             if (i < ctx->cfg_dirty_lo) ctx->cfg_dirty_lo = i;
@@ -476,7 +476,8 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
     mark_lines2(ctx, first, count);
     if (upload_cfg(ctx, stream)) return 1;
     for (int i = first; i < first + count; i++)
-        ctx->h_inp_late[i] = (kFusedNoise && ctx->h_cfg[i].lines2 && ctx->h_cfg[i].noise == 0) ? 1 : 0;
+        ctx->h_inp[i] = inp_pinned(ctx->h_inp[i]) ? kInpPinned
+                        : (kFusedNoise && ctx->h_cfg[i].lines2 && ctx->h_cfg[i].noise == 0) ? kInpLate : kInpWritten;
 #if (CRT_SYSTEM == CRT_SYSTEM_NTSCVHS)
     if (d_noise_terms) { // drop-in path: the terms were drawn from the process's libc on the host
         dim3 tgrid((kInputSize + 255) / 256, count);
@@ -527,19 +528,19 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
 
 int inp_from_analog(crtx_ctx *ctx, int first, int count, cudaStream_t stream)
 {
-    // one launch per run of monitors marked 1: a monitor outside them may carry a stale device flag, and its analog[] may
-    // have changed since
+    // one launch per run of late monitors: a monitor outside them may carry a stale device flag, and its analog[] may have
+    // changed since
     for (int lo = first; lo < first + count;) {
-        if (ctx->h_inp_late[lo] != 1) {
+        if (ctx->h_inp[lo] != kInpLate) {
             lo++;
             continue;
         }
         int hi = lo + 1;
-        while (hi < first + count && ctx->h_inp_late[hi] == 1) hi++;
+        while (hi < first + count && ctx->h_inp[hi] == kInpLate) hi++;
         k_inp_from_analog<<<hi - lo, 256, 0, stream>>>(ctx->d_state, ctx->d_analog, ctx->d_inp, lo);
         ctx->launches += 1;
         CUDA_TRY(cudaGetLastError());
-        for (int i = lo; i < hi; i++) ctx->h_inp_late[i] = 0;
+        for (int i = lo; i < hi; i++) ctx->h_inp[i] = kInpWritten;
         lo = hi;
     }
     return 0;
@@ -821,8 +822,7 @@ int crtx_create(crtx_ctx **out, int n)
     ctx->h_cfg.assign(n, MonCfg());
     memset(ctx->h_cfg.data(), 0, sizeof(MonCfg) * n);
     ctx->h_mod_staged.assign(n, 0);
-    ctx->h_inp_late.assign(n, 0);
-    ctx->h_inp_pinned.assign(n, 0);
+    ctx->h_inp.assign(n, kInpWritten);
     ctx->cfg_dirty_lo = 0;
     ctx->cfg_dirty_hi = n;
     ctx->tail_dirty_lo = 0;
@@ -1052,13 +1052,15 @@ signed char *crtx_analog(crtx_ctx *ctx, int i)
 signed char *crtx_inp(crtx_ctx *ctx, int i)
 {
     if (check_range(ctx, i, 1)) return NULL;
-    ctx->h_inp_pinned[i] = 1;
-    if (ctx->h_inp_late[i] == 1) {
+    const bool gone = inp_gone(ctx->h_inp[i]);
+    if (ctx->h_inp[i] == kInpLate) {
         if (cudaDeviceSynchronize() != cudaSuccess || inp_from_analog(ctx, i, 1, 0) || cudaDeviceSynchronize() != cudaSuccess) {
+            ctx->h_inp[i] = kInpPinned;
             fail("crtx_inp: making monitor %d's inp[] failed", i);
             return NULL;
         }
     }
+    ctx->h_inp[i] = gone ? kInpPinnedGone : kInpPinned; // (a gone inp[] stays unreadable until it is written again)
     return ctx->d_inp + (size_t) i * kSignalBytes;
 }
 
@@ -1066,7 +1068,7 @@ int crtx_read_signal(crtx_ctx *ctx, int i, int which, signed char *host, void *s
 {
     if (check_range(ctx, i, 1)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (which && ctx->h_inp_late[i] == 2)
+    if (which && inp_gone(ctx->h_inp[i]))
         return fail("monitor %d: inp[] of the last demodulate was decoded from analog[] (noise 0) and not kept, and a modulate has "
                     "rewritten analog[] since; crtx_inp(ctx, %d) keeps it from the next demodulate on", i, i);
     if (which && inp_from_analog(ctx, i, 1, st)) return 1;
@@ -1080,8 +1082,8 @@ int crtx_write_signal(crtx_ctx *ctx, int i, int which, const signed char *host, 
 {
     if (check_range(ctx, i, 1)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (which) ctx->h_inp_late[i] = 0;                          // (the caller's inp[] replaces it)
-    else if (inp_from_analog(ctx, i, 1, st)) return 1;           // (before the analog[] it is made from changes)
+    if (which) ctx->h_inp[i] = inp_pinned(ctx->h_inp[i]) ? kInpPinned : kInpWritten; // (the caller's inp[] replaces it)
+    else if (inp_from_analog(ctx, i, 1, st)) return 1;                                 // (before the analog[] it is made from changes)
     signed char *dst = (which ? ctx->d_inp : ctx->d_analog) + (size_t) i * kSignalBytes;
     CUDA_TRY(cudaMemcpyAsync(dst, host, kInputSize, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaStreamSynchronize(st));

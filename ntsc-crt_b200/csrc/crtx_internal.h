@@ -10,6 +10,16 @@
 
 #include "crt_records.h"
 
+namespace crt {
+// A monitor's inp[] after the calls so far.  At noise 0 a demodulate may leave it unwritten (crt_sync.cuh: inp_late): it is
+// late, made from analog[] when it is handed out, and gone once a modulate has rewritten that analog[].  Once crtx_inp has
+// handed out a raw pointer to it, it is pinned: k_sync writes it on every demodulate, so it is never late again.  A gone
+// inp[] that gets pinned stays unreadable until the next demodulate or write of it (kInpPinnedGone).
+enum InpState : unsigned char { kInpWritten, kInpLate, kInpGone, kInpPinned, kInpPinnedGone };
+inline bool inp_pinned(InpState s) { return s == kInpPinned || s == kInpPinnedGone; }
+inline bool inp_gone(InpState s) { return s == kInpGone || s == kInpPinnedGone; }
+} // namespace crt
+
 struct crtx_ctx {
     int n = 0;
     int device = 0;
@@ -38,10 +48,7 @@ struct crtx_ctx {
     std::vector<crt::MonCfg> h_cfg;
     std::vector<unsigned char> h_mod_staged; // per monitor: the last modulate encoded its picture with k_mod_picture_rgb_staged (crtx_get_paths)
     std::vector<crt::SrcCfg> scratch_src;
-    // per monitor, inp[] at noise 0 (crt_sync.cuh: inp_late): 1 = the last demodulate may have left it unwritten, to be made
-    // from analog[] when it is handed out; 2 = ... and a modulate has rewritten analog[] since, so it is gone
-    std::vector<unsigned char> h_inp_late;
-    std::vector<unsigned char> h_inp_pinned; // crtx_inp handed out a raw pointer: k_sync writes inp[] on every demodulate
+    std::vector<crt::InpState> h_inp; // per monitor
     int cfg_dirty_lo = 0, cfg_dirty_hi = 0;
     int tail_dirty_lo = 0, tail_dirty_hi = 0; // monitors whose output geometry changed: k_struct_tail rewrites the bytes behind their signals
     cudaEvent_t cfg_ready = nullptr;   // recorded behind the last configuration upload; launches on other streams wait on it

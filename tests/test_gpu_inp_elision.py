@@ -89,7 +89,8 @@ def test_poked_minus_128():
 
 def test_inp_after_a_later_modulate():
     """inp[] left unwritten is made from analog[]: once a modulate has rewritten analog[] it is gone, and reading it is an
-    error that says so rather than a wrong signal; a monitor whose inp[] pointer was taken keeps it"""
+    error that says so rather than a wrong signal, also after its pointer is taken then; a monitor whose inp[] pointer was
+    taken before keeps it"""
     from ntsc_crt_b200 import capi
     rig = S.BatchRig("ntsc", [dict(outw=640, outh=480, fmt=BGRA, noise=0, knobs=dict(blend=1, scanlines=1)) for _ in range(2)])
     try:
@@ -103,6 +104,9 @@ def test_inp_after_a_later_modulate():
         with pytest.raises(capi.CrtxError, match="monitor 0: inp"):
             rig.b.signal(0, "inp")
         assert np.array_equal(rig.b.signal(1, "inp"), want[1])
+        assert rig.b.inp_ptr(0)  # (pinned from now on, but what it points at is still gone)
+        with pytest.raises(capi.CrtxError, match="monitor 0: inp"):
+            rig.b.signal(0, "inp")
         rig.demodulate()
         _check(rig, "after the next demodulate")
     finally:
