@@ -298,8 +298,9 @@ constexpr int kModSChunk = 32;                     // samples per chunk of the s
 constexpr int kModSSpan = 192;                     // largest staged span the kernel accepts (incl. alignment slack)
 
 // Whether the staged picture kernel takes this source (the gather kernel takes the rest): the chunk's source span fits a
-// stage row, and the carrier has four or five samples per period.
-__host__ __device__ __forceinline__ bool mod_staged(const SrcCfg &s)
+// stage row, and the carrier has four or five samples per period.  The host decides it once per modulate and passes it on
+// in SrcCfg::staged (crtx.cu: modulate_launch); the kernels read only that.
+inline bool mod_staged(const SrcCfg &s)
 {
     int destw, desth;
     picture_size(s, destw, desth);
@@ -343,8 +344,7 @@ __device__ __forceinline__ void carrier_lane(const SrcCfg &s, int crow, bool col
 // (256, 2): its shared memory fits two CTAs per SM; a higher target spills the 64-bit row addresses
 __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb(const SrcCfg *__restrict__ srcs,
                                                          const MonCfg *__restrict__ cfgs,
-                                                         signed char *__restrict__ analog_base, int first,
-                                                         int skip_staged)
+                                                         signed char *__restrict__ analog_base, int first)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -357,7 +357,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb(const SrcCfg *__rest
 
     const int bpp = bpp_of(s.format);
     if (bpp == 0) return;
-    if (skip_staged && mod_staged(s)) return; // done by k_mod_picture_rgb_staged
+    if (s.staged) return; // done by k_mod_picture_rgb_staged
     int destw, desth, xo, yo;
     picture_size(s, destw, desth);
     if (destw <= 0 || desth <= 0 || s.w <= 0 || s.h <= 0) return;
@@ -449,8 +449,8 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb(const SrcCfg *__rest
 // shared-memory latency and no transposition of the input is needed.  Which source pixel a sample
 // reads is tabulated once per CTA.  Finished samples are packed 4 to a word and written back in
 // windows aligned to 32-byte sectors (put, below).
-// Usable when the chunk's source span fits a stage row; other monitors return at once and are
-// handled by k_mod_picture_rgb (gather variant), which in turn skips the ones done here.
+// Usable when the chunk's source span fits a stage row (mod_staged).  The host marks the sources it takes (SrcCfg::staged);
+// other monitors return at once and are handled by k_mod_picture_rgb (gather variant), which in turn skips the marked ones.
 // The source image must be readable up to the next 16-byte boundary past its last pixel
 // (true of any cudaMalloc / torch allocation; include/crtx_batch.h).  A row's copy covers the 16-byte aligned superset
 // of its span, which may take in bytes of the padding between rows: they land in the stage and are never used.
@@ -524,7 +524,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const SrcCfg s = srcs[blockIdx.x];
-    if (!mod_staged(s) || s.format != FMT || (s.as_color != 0) != COLOR) return;
+    if (!s.staged || s.format != FMT || (s.as_color != 0) != COLOR) return;
     const MonCfg cfg = cfgs[first + blockIdx.x];
     signed char *analog = analog_base + (size_t) (first + blockIdx.x) * kSignalBytes;
 

@@ -139,15 +139,6 @@ template <bool FAST> constexpr int lines_smem() { return kLinesWarps * lines_war
 // kMaxOutw, where a single sample can still not overrun the 32-column tile ring) takes MAXP == 0.
 constexpr int kMaxOutw = 8192;
 
-struct LinesGeom { // uniform over a launch: host groups monitors by these (crtx.cu)
-    int outw, out_format, bpp, blend;
-    int pitch; // bytes between output rows (MonCfg::out_pitch, shared by every monitor of the launch)
-    int pass; // -1: every line; -2: only the last line of each shared-row run; >= 0: lines at this run position (level)
-    int rnd; // 32768, passed as an argument so that it lives in a register (see pole())
-    int dx;  // ((AV_LEN - 1) << 12) / outw (crt_core.c:527), computed by the host: no division in the kernels
-    int line_lo, line_hi; // decoded lines [lo, hi) this launch may touch (scanline-block sharding across ranks)
-};
-
 // Whether a line pass decodes decoded line k, whose record is `l` (a LineRec, or anything with its beg, run_pos and
 // run_last): a line of the field (k < CRT_LINES) that the field shows (beg >= 0), inside the launch's window
 // [line_lo, line_hi), in the launch's pass.  (One flat condition: the kernels' code depends on its shape.)

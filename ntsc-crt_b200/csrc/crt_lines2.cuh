@@ -2,7 +2,7 @@
 // actually use: stock equaliser gains on their exact fast path (see eq_step), 4-byte pixels, 16-byte aligned rows,
 // an output about as wide as the line has samples (kL2MinDx4096 .. kL2MaxOutw).  Everything else -- 3-byte pixels,
 // very narrow or very wide outputs, the wrap-exact generic equaliser, rows shared by several lines, the PV-1000 --
-// stays with k_lines (crt_lines.cuh); the host picks per launch (crtx.cu: lines2_eligible).
+// stays with k_lines (crt_lines.cuh); the host picks once per run of a demodulate's line plan (crtx.cu: plan_lines).
 //
 // Same shape as k_lines -- one LANE carries one scanline through the equalisers -- with three changes:
 //   * a CTA is 15 warps = 480 lane-lines = TWO monitors.  240 lines are 7.5 warps: k_lines leaves half a warp

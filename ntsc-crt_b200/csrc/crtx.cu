@@ -129,10 +129,10 @@ static void launch_lines_k(crtx_ctx *ctx, int count, int lo, const LinesGeom &ge
 // IIR decoder, 4-byte pixels, every line owning its rows, a width the pixel ring covers, rows that start on 16-byte
 // boundaries (the run's pitch and every image's address multiples of 16).
 #if CRTX_HAS_LINES2
-static bool lines2_eligible(const crtx_ctx *ctx, int count, int lo, const LinesGeom &geo)
+static bool lines2_eligible(const crtx_ctx *ctx, int count, int lo, const LinesGeom &geo, const LinePasses &passes)
 {
     if (!ctx->opt_lines2) return false;
-    if (geo.bpp != 4 || geo.pass != -1 || !lines2_geometry_ok(geo.outw) || (geo.pitch & 15)) return false;
+    if (geo.bpp != 4 || passes.first != -1 || !lines2_geometry_ok(geo.outw) || (geo.pitch & 15)) return false;
     for (int i = lo; i < lo + count; i++)
         if (reinterpret_cast<uintptr_t>(ctx->h_cfg[i].out) & 15) return false;
     return true;
@@ -149,11 +149,12 @@ static void launch_lines2(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo
     });
 }
 #else
-static bool lines2_eligible(const crtx_ctx *, int, int, const LinesGeom &) { return false; }
+static bool lines2_eligible(const crtx_ctx *, int, int, const LinesGeom &, const LinePasses &) { return false; }
 static void launch_lines2(crtx_ctx *, int, int, const LinesGeom &, cudaStream_t) {}
 #endif
 
-static void launch_lines(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo, cudaStream_t stream)
+// one launch of the line pass geo.pass: k_lines2 where the line plan chose it (`lines2`), else the build's line kernel
+static void launch_lines(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo, bool lines2, cudaStream_t stream)
 {
     if (kBloom) { // CRT_DO_BLOOM build: per-line resampling step, one kernel for every format (crt_bloom.cuh)
         k_lines_bloom<<<dim3(kBloomGroups, count), kBloomWarps * 32, kBloomSmem, stream>>>(
@@ -161,7 +162,7 @@ static void launch_lines(crtx_ctx *ctx, int count, int lo, const LinesGeom &geo,
         ctx->launches += 1;
         return;
     }
-    if (lines2_eligible(ctx, count, lo, geo)) launch_lines2(ctx, count, lo, geo, stream);
+    if (lines2) launch_lines2(ctx, count, lo, geo, stream);
     else launch_lines_k<true>(ctx, count, lo, geo, stream);
     launch_lines_k<false>(ctx, count, lo, geo, stream); // the monitors k_sync flagged for the wrap-exact equaliser
 }
@@ -318,12 +319,24 @@ struct LaunchTimer {
     }
 };
 
-int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cudaStream_t stream)
+int modulate_launch(crtx_ctx *ctx, int first, int count, SrcCfg *src, cudaStream_t stream)
 {
     if (check_range(ctx, first, count)) return 1;
     if (count == 0) return 0;
     for (int i = first; i < first + count; i++)
         if (ctx->h_inp[i] == kInpLate) ctx->h_inp[i] = kInpGone; // (the analog[] it would be made from is about to change)
+#if CRT_B200_BANDLIMITED
+    // The picture kernel of every source, chosen here and nowhere else: the staged one takes what mod_staged accepts
+    // (SrcCfg::staged), the gather one the rest, and each returns for the other's.  The gather kernel only runs when it has
+    // a source to encode, or for all of them when staging is off, so the usual call saves a launch.
+    const bool staged = ctx->opt_mod_staged != 0;
+    bool gather = !staged;
+    for (int i = 0; i < count; i++) {
+        src[i].staged = (staged && mod_staged(src[i])) ? 1 : 0;
+        if (bpp_of(src[i].format) != 0 && !src[i].staged) gather = true;
+        ctx->h_mod_staged[first + i] = (unsigned char) src[i].staged;
+    }
+#endif
     if (upload_cfg(ctx, stream)) return 1;
     CUDA_TRY(cudaMemcpyAsync(ctx->d_src + first, src, sizeof(SrcCfg) * count, cudaMemcpyHostToDevice, stream));
 #if (CRT_SYSTEM == CRT_SYSTEM_NTSCVHS)
@@ -356,17 +369,7 @@ int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cuda
                                                               first);
         ctx->launches += 1;
     }
-#else
-    // (the staged kernel steps four samples per carrier period: not for the PV-1000's five, which takes the gather kernel)
-    const bool staged = ctx->opt_mod_staged && (kCc == 4 || kCc == 5);
-    // The gather kernel only runs for sources the staged one cannot take (their span does not fit a stage row), or for all of
-    // them when staging is off: the host can tell (mod_staged is a pure function of the settings), so the usual call saves a launch.
-    bool gather = !staged;
-    for (int i = 0; i < count; i++) {
-        const bool takes = bpp_of(src[i].format) != 0 && staged && mod_staged(src[i]);
-        if (bpp_of(src[i].format) != 0 && staged && !takes) gather = true;
-        ctx->h_mod_staged[first + i] = takes ? 1 : 0;
-    }
+#else // (CRT_B200_BANDLIMITED)
     {
         LaunchTimer lt(ctx, stream, 0);
         k_mod_skeleton_rgb<<<count, 256, 0, stream>>>(ctx->d_src + first, ctx->d_state, ctx->d_analog, first);
@@ -383,8 +386,7 @@ int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cuda
             }
         }
         if (gather) {
-            k_mod_picture_rgb<<<count, 256, kModSmem, stream>>>(ctx->d_src + first, ctx->d_cfg, ctx->d_analog, first,
-                                                                staged ? 1 : 0);
+            k_mod_picture_rgb<<<count, 256, kModSmem, stream>>>(ctx->d_src + first, ctx->d_cfg, ctx->d_analog, first);
             ctx->launches += 1;
         }
     }
@@ -400,10 +402,6 @@ int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cuda
 //   fewer rows, no blend        only the last line of each run of lines on one row survives: one pass of those (-2)
 //   fewer rows, blend           one pass per position in the runs
 //   rows above kMonotonicSpan   lines far apart share rows: one pass per level, blend or not
-struct LinePasses {
-    int first, count;
-};
-
 static LinePasses line_passes(const MonCfg &c)
 {
     const unsigned rows = row_span(c);
@@ -435,7 +433,7 @@ static int run_end(const crtx_ctx *ctx, int lo, int end)
 static LinesGeom run_geom(const crtx_ctx *ctx, int lo)
 {
     const MonCfg &c0 = ctx->h_cfg[lo];
-    LinesGeom geo;
+    LinesGeom geo = {};
     geo.outw = c0.outw;
     geo.out_format = c0.out_format;
     geo.bpp = c0.bpp;
@@ -445,27 +443,32 @@ static LinesGeom run_geom(const crtx_ctx *ctx, int lo)
     geo.dx = c0.outw > 0 ? ((kAvLen - 1) << 12) / c0.outw : 0;
     geo.line_lo = ctx->opt_line_lo;
     geo.line_hi = ctx->opt_line_hi;
-    geo.pass = line_passes(c0).first;
     return geo;
 }
 
-// MonCfg::lines2 of every monitor in [first, first + count): whether this demodulate's line pass is k_lines2, which then
-// decodes from analog[] where k_sync leaves inp[] unwritten (crt_sync.cuh: inp_late), and no raw pointer to the monitor's
-// inp[] was handed out.  A change travels with the next upload_cfg.
-static void mark_lines2(crtx_ctx *ctx, int first, int count)
+// The line plan of a demodulate of [first, first + count), made once before any launch: its runs, each with its geometry,
+// its passes and its kernel, into ctx->scratch_runs.  MonCfg::lines2 comes from the same plan: k_sync leaves inp[] unwritten
+// (crt_sync.cuh: inp_late) only for monitors k_lines2 then decodes from analog[], and never for one whose raw inp[] pointer
+// was handed out.  A change of the flag travels with the next upload_cfg.
+static void plan_lines(crtx_ctx *ctx, int first, int count)
 {
+    ctx->scratch_runs.clear();
     for (int lo = first; lo < first + count;) {
-        const int hi = run_end(ctx, lo, first + count);
-        const LinesGeom geo = run_geom(ctx, lo);
-        const bool eligible = lines2_eligible(ctx, hi - lo, lo, geo);
-        for (int i = lo; i < hi; i++) {
-            const int want = (eligible && !inp_pinned(ctx->h_inp[i])) ? 1 : 0;
+        LineRun r;
+        r.lo = lo;
+        r.hi = run_end(ctx, lo, first + count);
+        r.geo = run_geom(ctx, lo);
+        r.passes = line_passes(ctx->h_cfg[lo]);
+        r.lines2 = lines2_eligible(ctx, r.hi - r.lo, r.lo, r.geo, r.passes);
+        for (int i = r.lo; i < r.hi; i++) {
+            const int want = (r.lines2 && !inp_pinned(ctx->h_inp[i])) ? 1 : 0;
             if (ctx->h_cfg[i].lines2 == want) continue;
             ctx->h_cfg[i].lines2 = want;
             if (i < ctx->cfg_dirty_lo) ctx->cfg_dirty_lo = i;
             if (i + 1 > ctx->cfg_dirty_hi) ctx->cfg_dirty_hi = i + 1;
         }
-        lo = hi;
+        ctx->scratch_runs.push_back(r);
+        lo = r.hi;
     }
 }
 
@@ -473,7 +476,7 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
 {
     if (check_range(ctx, first, count)) return 1;
     if (count == 0) return 0;
-    mark_lines2(ctx, first, count);
+    plan_lines(ctx, first, count);
     if (upload_cfg(ctx, stream)) return 1;
     for (int i = first; i < first + count; i++)
         ctx->h_inp[i] = inp_pinned(ctx->h_inp[i]) ? kInpPinned
@@ -511,16 +514,13 @@ int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, 
         k_bloom<<<count, 256, 0, stream>>>(ctx->d_cfg, ctx->d_lines, ctx->d_inp, static_cast<BloomLine *>(ctx->d_bloom), first);
         ctx->launches += 1;
     }
-    for (int lo = first; lo < first + count;) {
-        const int hi = run_end(ctx, lo, first + count);
-        LinesGeom geo = run_geom(ctx, lo);
+    for (const LineRun &r : ctx->scratch_runs) {
+        LinesGeom geo = r.geo;
         LaunchTimer lt(ctx, stream, 4);
-        const LinePasses passes = line_passes(ctx->h_cfg[lo]);
-        for (int p = 0; p < passes.count; p++) {
-            geo.pass = passes.first + p;
-            launch_lines(ctx, hi - lo, lo, geo, stream);
+        for (int p = 0; p < r.passes.count; p++) {
+            geo.pass = r.passes.first + p;
+            launch_lines(ctx, r.hi - r.lo, r.lo, geo, r.lines2, stream);
         }
-        lo = hi;
     }
     CUDA_TRY(cudaGetLastError());
     return 0;
@@ -822,6 +822,7 @@ int crtx_create(crtx_ctx **out, int n)
     ctx->h_cfg.assign(n, MonCfg());
     memset(ctx->h_cfg.data(), 0, sizeof(MonCfg) * n);
     ctx->h_mod_staged.assign(n, 0);
+    ctx->scratch_runs.reserve(n); // (a demodulate plans at most one run per monitor)
     ctx->h_inp.assign(n, kInpWritten);
     ctx->cfg_dirty_lo = 0;
     ctx->cfg_dirty_hi = n;
@@ -1048,7 +1049,7 @@ signed char *crtx_analog(crtx_ctx *ctx, int i)
 }
 
 // The caller may read or write inp[] through the pointer at any time: from now on k_sync writes it on every demodulate
-// (mark_lines2), and what the last demodulate left unwritten is made now, after the work already queued on any stream.
+// (plan_lines), and what the last demodulate left unwritten is made now, after the work already queued on any stream.
 signed char *crtx_inp(crtx_ctx *ctx, int i)
 {
     if (check_range(ctx, i, 1)) return NULL;
@@ -1205,7 +1206,7 @@ int crtx_frames_host(crtx_ctx *ctx, int first, int count, const crtx_source *src
         if (!out_host || !out_host[i]) continue;
         const int row_bytes = c.outw * c.bpp;
         void *map = (ctx->opt_host_rows && row_bytes > 0 && (c.out_pitch & 15) == 0 && (reinterpret_cast<uintptr_t>(c.out) & 15) == 0
-                     && row_span(c) >= (unsigned) kLines && row_span(c) <= kMonotonicSpan) // every row written by one line
+                     && line_passes(c).first == -1) // every row written by one line
                         ? host_mapping(out_host[i]) : NULL;
         if (map && (reinterpret_cast<uintptr_t>(map) & 15) == 0) {
             maps[i] = static_cast<unsigned char *>(map);

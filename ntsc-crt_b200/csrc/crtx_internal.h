@@ -18,6 +18,20 @@ namespace crt {
 enum InpState : unsigned char { kInpWritten, kInpLate, kInpGone, kInpPinned, kInpPinnedGone };
 inline bool inp_pinned(InpState s) { return s == kInpPinned || s == kInpPinnedGone; }
 inline bool inp_gone(InpState s) { return s == kInpGone || s == kInpPinnedGone; }
+
+// The line passes of a run of monitors: LinesGeom::pass takes first, first + 1, .. first + count - 1 (crtx.cu: line_passes)
+struct LinePasses {
+    int first, count;
+};
+
+// One run of a demodulate's line plan (crtx.cu: plan_lines): monitors [lo, hi) share the output geometry `geo` (its pass
+// is set per launch) and are decoded by `passes` launches of k_lines2 (`lines2`) or of the build's line kernel
+struct LineRun {
+    int lo, hi;
+    LinesGeom geo;
+    LinePasses passes;
+    bool lines2;
+};
 } // namespace crt
 
 struct crtx_ctx {
@@ -48,6 +62,7 @@ struct crtx_ctx {
     std::vector<crt::MonCfg> h_cfg;
     std::vector<unsigned char> h_mod_staged; // per monitor: the last modulate encoded its picture with k_mod_picture_rgb_staged (crtx_get_paths)
     std::vector<crt::SrcCfg> scratch_src;
+    std::vector<crt::LineRun> scratch_runs; // demodulate_launch's line plan
     std::vector<crt::InpState> h_inp; // per monitor
     int cfg_dirty_lo = 0, cfg_dirty_hi = 0;
     int tail_dirty_lo = 0, tail_dirty_hi = 0; // monitors whose output geometry changed: k_struct_tail rewrites the bytes behind their signals
@@ -75,7 +90,8 @@ namespace crt {
 inline long long src_row_bytes(int format, int w) { return (long long) w * (kIsNes ? 2 : bpp_of(format)); }
 int fail(const char *fmt, ...);
 void fill_src(SrcCfg *d, const crtx_source *s);
-int modulate_launch(crtx_ctx *ctx, int first, int count, const SrcCfg *src, cudaStream_t stream);
+// sets SrcCfg::staged of every src[i] before it uploads them
+int modulate_launch(crtx_ctx *ctx, int first, int count, SrcCfg *src, cudaStream_t stream);
 // d_noise_terms: VHS only -- per-sample noise term already drawn on the host from libc rand()
 int demodulate_launch(crtx_ctx *ctx, int first, int count, cudaStream_t stream, const short *d_noise_terms);
 // inp[] of monitors [first, first + count) made from analog[] where the last demodulate left it (ordered on `stream`)

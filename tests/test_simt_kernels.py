@@ -27,6 +27,7 @@ import test_gpu_edges as _edges  # noqa: E402
 import test_gpu_fullsize as _fullsize  # noqa: E402
 import test_gpu_fuzz as _fuzz  # noqa: E402
 import test_gpu_guard_edges as _guard  # noqa: E402
+import test_gpu_inp_elision as _elision  # noqa: E402
 import test_gpu_lines2 as _lines2  # noqa: E402
 import test_gpu_lineshard as _lineshard  # noqa: E402
 import test_gpu_parity as _parity  # noqa: E402
@@ -111,6 +112,10 @@ _adopt(_vhs, "vhs")
 test_cli_unmodified_cli_driver_is_byte_identical = _cli.test_unmodified_cli_driver_is_byte_identical
 _adopt(_still, "still")
 test_vconv_unmodified_video_convert_runs_against_the_library = _vconv.test_unmodified_video_convert_runs_against_the_library
+# k_sync leaving inp[] unwritten and the line pass that then decodes from analog[] must agree (not the 264-monitor batch)
+test_elision_mixed_batch = _elision.test_mixed_batch
+test_elision_poked_minus_128 = _elision.test_poked_minus_128
+test_elision_inp_after_a_later_modulate = _elision.test_inp_after_a_later_modulate
 
 
 def _bare(fn):
