@@ -13,6 +13,10 @@
  * The library variant fixes the emulated system, as in the reference (compile-time
  * CRT_SYSTEM): query it with crtx_system().
  *
+ * The VHS build draws its noise from a per-monitor replica of glibc's rand(): crtx_seed sets it as srand() would,
+ * crtx_get_rand / crtx_set_rand save and restore it, and crtx_skip_fields advances it over whole fields without
+ * running them (how the time-parallel video path starts each segment of a sequence where the sequential loop would).
+ *
  * All functions return 0 on success, non-zero on failure (crtx_last_error() explains);
  * they never fall back to a CPU path.
  */
@@ -110,6 +114,24 @@ int crtx_set_monitors(crtx_ctx *ctx, int first, int count, const crtx_monitor *m
 int crtx_set_state(crtx_ctx *ctx, int first, int count, const crtx_state *s, void *stream);
 int crtx_get_state(crtx_ctx *ctx, int first, int count, crtx_state *s, void *stream);
 int crtx_seed(crtx_ctx *ctx, int first, int count, unsigned seed); /* VHS libc-rand() replica */
+
+/* The VHS build's rand() replica, one per monitor: glibc's TYPE_3 generator (o[n] = o[n-31] + o[n-3] mod 2^32, rand()
+ * returns o[n] >> 1), whose whole state is its last 31 raw values.  Saving and restoring it lets a VHS monitor be
+ * checkpointed, cloned or moved to another process.  `words` holds CRTX_RAND_WORDS words per monitor in chronological
+ * order, oldest first: the order the recurrence reads them, not glibc's ring.  From glibc's struct random_data (after
+ * srandom_r / initstate_r with TYPE_3) that order is words[j] = state[(fptr - state + j) % 31], j = 0 .. 30, and
+ * rptr - state = (fptr - state + 28) % 31.
+ * crtx_get_rand synchronises `stream`, like crtx_get_state; crtx_set_rand is ordered on `stream`, like crtx_set_state.
+ * crtx_skip_fields advances monitor first + k's replica by the draws of fields[k] crtx_modulate + crtx_demodulate pairs,
+ * asynchronously on `stream`, without touching a signal: what a field draws depends on its own values alone, never on the
+ * images, the noise or the knobs -- given sources and an output of known pixel formats (an unknown source format draws no
+ * aberration, an unknown output format nothing) and do_aberration as the sources set it.  A negative field count is an
+ * error, and leaves every monitor as it was.  Builds other than VHS draw nothing from rand(): all three calls fail there,
+ * and say so in crtx_last_error(). */
+#define CRTX_RAND_WORDS 31
+int crtx_get_rand(crtx_ctx *ctx, int first, int count, unsigned *words /* count * CRTX_RAND_WORDS */, void *stream);
+int crtx_set_rand(crtx_ctx *ctx, int first, int count, const unsigned *words, void *stream);
+int crtx_skip_fields(crtx_ctx *ctx, int first, int count, const int *fields, int do_aberration, void *stream);
 
 /* DEVICE pointers to monitor i's signal buffers (CRT_INPUT_SIZE + slack bytes each) */
 signed char *crtx_analog(crtx_ctx *ctx, int i);

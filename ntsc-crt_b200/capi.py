@@ -83,7 +83,7 @@ CRT_EXPORTS = ("crt_init", "crt_resize", "crt_reset", "crt_modulate", "crt_demod
                "crt_bpp4fmt", "crt_sincos14")
 CRTX_EXPORTS = ("crtx_system", "crtx_chroma_pattern", "crtx_nes_border", "crtx_do_vsync", "crtx_do_hsync", "crtx_hres", "crtx_input_size", "crtx_lines",
                 "crtx_cc_vper", "crtx_create", "crtx_destroy", "crtx_set_monitors", "crtx_set_state",
-                "crtx_get_state", "crtx_seed", "crtx_analog", "crtx_inp", "crtx_read_signal",
+                "crtx_get_state", "crtx_seed", "crtx_get_rand", "crtx_set_rand", "crtx_skip_fields", "crtx_analog", "crtx_inp", "crtx_read_signal",
                 "crtx_write_signal", "crtx_modulate",
                 "crtx_demodulate", "crtx_frames_host", "crtx_get_lines", "crtx_get_paths", "crtx_launch_count",
                 "crtx_lines2_count", "crtx_set_option", "crtx_get_timing", "crtx_last_error")
@@ -110,6 +110,9 @@ def load(variant):
     lib.crtx_set_state.argtypes = [vp, ip, ip, C.POINTER(State), vp]
     lib.crtx_get_state.argtypes = [vp, ip, ip, C.POINTER(State), vp]
     lib.crtx_seed.argtypes = [vp, ip, ip, C.c_uint]
+    lib.crtx_get_rand.argtypes = [vp, ip, ip, C.POINTER(C.c_uint), vp]
+    lib.crtx_set_rand.argtypes = [vp, ip, ip, C.POINTER(C.c_uint), vp]
+    lib.crtx_skip_fields.argtypes = [vp, ip, ip, C.POINTER(C.c_int), ip, vp]
     lib.crtx_analog.argtypes = [vp, ip]
     lib.crtx_analog.restype = vp
     lib.crtx_inp.argtypes = [vp, ip]
@@ -238,6 +241,29 @@ class Batch:
         """VHS: put the monitors' rand() replica in the state srand(seed) leaves glibc in."""
         count = self.n - first if count is None else count
         self._check(self.lib.crtx_seed(self._ctx, first, count, seed))
+
+    RAND_WORDS = 31  # CRTX_RAND_WORDS
+
+    def get_rand(self, first=0, count=None, stream=0):
+        """VHS: the monitors' rand() replica as a (count, 31) uint32 array, each row the generator's last 31 raw values,
+        oldest first (synchronises the stream)"""
+        import numpy as np
+        count = self.n - first if count is None else count
+        words = np.zeros((count, self.RAND_WORDS), dtype=np.uint32)
+        self._check(self.lib.crtx_get_rand(self._ctx, first, count, words.ctypes.data_as(C.POINTER(C.c_uint)), stream))
+        return words
+
+    def set_rand(self, words, first=0, stream=0):
+        """VHS: set monitors [first, first + len(words)) to the generator states get_rand returned"""
+        import numpy as np
+        words = np.ascontiguousarray(words, dtype=np.uint32).reshape(-1, self.RAND_WORDS)
+        self._check(self.lib.crtx_set_rand(self._ctx, first, words.shape[0], words.ctypes.data_as(C.POINTER(C.c_uint)), stream))
+
+    def skip_fields(self, fields, do_aberration=0, first=0, stream=0):
+        """VHS: advance monitor first + k's replica by the draws of fields[k] modulate + demodulate pairs (known pixel
+        formats, do_aberration as the sources would set it), without running them"""
+        arr = (C.c_int * len(fields))(*[int(f) for f in fields])
+        self._check(self.lib.crtx_skip_fields(self._ctx, first, len(fields), arr, int(do_aberration), stream))
 
     def get_lines(self, i, stream=0):
         t = (Line * self.spec.lines)()

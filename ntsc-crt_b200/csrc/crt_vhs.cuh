@@ -60,6 +60,7 @@ struct VhsRand { // generator state: the last 31 raw values, oldest first
 struct VhsJump { // powers of the transition matrix, [level][row][col], applied as new = A * old
     unsigned bulk[kVhsLevels][31][31]; // (M^(2 * kVhsRun))^(2^level)
     unsigned tail[kVhsLevels][31][31]; // (M^kVhsTailRun)^(2^level)
+    unsigned field[2][31][31];         // M^(ab + 1 + 2 * kVhsBulk): a field's draws before its tail, ab = the aberration draw
 };
 
 // one draw on a chronological state held in shared/global memory (used for the odd single draws)
@@ -115,6 +116,79 @@ __device__ __forceinline__ void vhs_apply(unsigned *to, const unsigned (*A)[31],
         to[tid] = acc;
     }
     __syncthreads();
+}
+
+// draws per regular sample (x >= 1) of signal line `line` where that number does not depend on the data, else 0: within
+// the line the first test of sample x >= 1 is (draw % 20) >= need (crt_core.c:350 with i = line * HRES + x)
+__device__ __forceinline__ int vhs_fixed_draws(int line)
+{
+    const int need = (kInputSize / kHres - 6) - line;
+    return (need > 19) ? 2 : (need <= 0) ? 3 : 0;
+}
+
+// One line of the tail walk, samples xa .. kHres - 1 of signal line `line` (i0 = line * kHres + xa), whose first draw is
+// raw[D]: win = raw[D ..], *s_start = the position of its first regular sample in win, and where the line's draw count
+// depends on the data, jt[k][p] = the position 2^k regular samples after position p (k < kVhsJLevels).  Within a line
+// the first test is the same function of its draw for every sample except x == 0 (its bound is a multiple of the line
+// length), so x == 0 is stepped on its own and the regular samples start at x0 = 1 (or at xa > 0).  k_vhs_skip walks
+// with these tables; k_noise_vhs runs the same steps inline, interleaved with its chunk table, which keeps its machine
+// code as it was (the compiler schedules the shared version differently there).
+__device__ __forceinline__ void vhs_line_tables(unsigned *win, unsigned short *jt, int *s_start, const unsigned *raw, int D,
+                                                int i0, int xa, int line, int fixed, int tid)
+{
+    { // all of a thread's window loads in flight together
+        constexpr int kPer = (kVhsWin + 8 + kVhsThreads - 1) / kVhsThreads;
+        unsigned v[kPer];
+#pragma unroll
+        for (int u = 0; u < kPer; u++) {
+            const int q = tid + u * kVhsThreads;
+            v[u] = (q < kVhsWin + 8 && D + q < kVhsTailRaw) ? raw[D + q] : 0u;
+        }
+#pragma unroll
+        for (int u = 0; u < kPer; u++) {
+            const int q = tid + u * kVhsThreads;
+            if (q < kVhsWin + 8) win[q] = v[u];
+        }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int p = 0;
+        if (xa == 0) p = 2 + (vhs_test1(i0, win[1] >> 1) ? 1 : 0);
+        *s_start = p; // position of the first "regular" sample
+    }
+    if (!fixed) {
+        const int irep = line * kHres + 1;
+        for (int p = tid; p < kVhsWin + 8; p += kVhsThreads)
+            jt[p] = (unsigned short) ((p + 3 < kVhsWin) ? p + 2 + (vhs_test1(irep, win[p + 1] >> 1) ? 1 : 0) : kVhsWin);
+        __syncthreads();
+        for (int k = 1; k < kVhsJLevels; k++) { // jt[k][p] = 2^k-th successor
+            unsigned short *prev = jt + (k - 1) * (kVhsWin + 8), *cur = jt + k * (kVhsWin + 8);
+#pragma unroll 4
+            for (int p = tid; p < kVhsWin + 8; p += kVhsThreads) cur[p] = prev[min((int) prev[p], kVhsWin)];
+            __syncthreads();
+        }
+    }
+}
+
+// The tail CTA's raw stream: from the state at the start of the tail in states[0], raw[0 .. kVhsTailRaw) = the next
+// kVhsTailRaw raw values of the generator (jumps of kVhsTailRun values spread the start states over the threads).
+// Ends with the block synchronised; `states` may then be overlaid.
+__device__ __forceinline__ void vhs_tail_stream(unsigned (*states)[32], const VhsJump *jump, unsigned *raw, int tid, unsigned *Am)
+{
+    vhs_spread_states(states, jump->tail, tid, Am);
+    {
+        unsigned h[31];
+#pragma unroll
+        for (int j = 0; j < 31; j++) h[j] = states[tid][j];
+        for (int it = 0; it < kVhsTailRun / 31; it++) {
+#pragma unroll
+            for (int d = 0; d < 31; d++) {
+                h[d] += h[(d + 28) % 31];
+                raw[tid * kVhsTailRun + it * 31 + d] = h[d];
+            }
+        }
+    }
+    __syncthreads(); // (block-wide: the stream is visible to every thread; `states` may now be overlaid)
 }
 
 __global__ void __launch_bounds__(kVhsThreads, 4) k_noise_vhs(const MonCfg *__restrict__ cfgs, MonState *__restrict__ states_mon,
@@ -230,29 +304,14 @@ __global__ void __launch_bounds__(kVhsThreads, 4) k_noise_vhs(const MonCfg *__re
             __syncthreads();
         }
     }
-    vhs_spread_states(states, jump->tail, tid, s_mat);
-    {
-        unsigned h[31];
-#pragma unroll
-        for (int j = 0; j < 31; j++) h[j] = states[tid][j];
-        for (int it = 0; it < kVhsTailRun / 31; it++) {
-#pragma unroll
-            for (int d = 0; d < 31; d++) {
-                h[d] += h[(d + 28) % 31];
-                raw[tid * kVhsTailRun + it * 31 + d] = h[d];
-            }
-        }
-    }
-    __syncthreads(); // (block-wide: the stream is visible to every thread; `states` may now be overlaid)
+    vhs_tail_stream(states, jump, raw, tid, s_mat);
 
     // ---- tail walk, one signal line (or the partial first one) at a time
     const int wobble = s_wobble;
     int D = 0;            // raw values consumed so far in the tail
     for (int i0 = kVhsBulk; i0 < kInputSize;) {
         const int line = i0 / kHres, xa = i0 - line * kHres, nx = kHres - xa; // samples xa .. 909 of this line
-        // for x >= 1 of this line the first test is (draw % 20) >= need (crt_core.c:350 with i = line * HRES + x)
-        const int need = (kInputSize / kHres - 6) - line;
-        const int fixed = (need > 19) ? 2 : (need <= 0) ? 3 : 0; // draws per regular sample when it is not data dependent
+        const int fixed = vhs_fixed_draws(line);
         { // all of a thread's window loads in flight together
             constexpr int kPer = (kVhsWin + 8 + kVhsThreads - 1) / kVhsThreads;
             unsigned v[kPer];
@@ -365,6 +424,63 @@ constexpr int kVhsSmemBulk = (257 * 32 * 4 > kVhsRuns * kVhsSlice * 2) ? 257 * 3
 constexpr int kVhsSmemTail = (kVhsWin + 8) * 4 + kVhsJLevels * (kVhsWin + 8) * 2 + kVhsChunks * 4 + 16;
 constexpr int kVhsSmem = (kVhsSmemBulk > kVhsSmemTail ? kVhsSmemBulk : kVhsSmemTail) > 257 * 32 * 4
                              ? (kVhsSmemBulk > kVhsSmemTail ? kVhsSmemBulk : kVhsSmemTail) : 257 * 32 * 4;
+constexpr int kVhsSkipSmem = kVhsSmemTail > 257 * 32 * 4 ? kVhsSmemTail : 257 * 32 * 4; // the tail CTA's part of kVhsSmem
+
+// Advance monitor first + b's replica by fields[b] modulate + demodulate pairs, b = blockIdx.x, without a signal: what a
+// field draws depends on its own values alone, never on the images, the noise or the knobs.  Per field: the draws
+// before the tail -- [the aberration draw, ab] + the wobble + two per bulk sample -- are one matrix (VhsJump::field[ab]);
+// the tail's raw stream is generated as k_noise_vhs's tail CTA does, and walked line by line with the same tables: the
+// line's draw count is s_start + fixed * samples where it does not depend on the data, else the position the successor
+// tables give after its last sample.  The next field starts from the last 31 raw values consumed.  One CTA per monitor:
+// each field's count depends on that field's values.  The state after the call goes to rands_next (k_vhs_commit).
+__global__ void __launch_bounds__(kVhsThreads) k_vhs_skip(const int *__restrict__ fields, const VhsRand *__restrict__ rands,
+                                                          VhsRand *__restrict__ rands_next, const VhsJump *__restrict__ jump,
+                                                          unsigned *__restrict__ raw_base, int ab, int first)
+{
+    extern __shared__ __align__(16) unsigned char vsm[];
+    unsigned (*states)[32] = reinterpret_cast<unsigned (*)[32]>(vsm);                 // [257][32]
+    unsigned *win = reinterpret_cast<unsigned *>(vsm);                                  // walk: [kVhsWin + 8]
+    unsigned short *jt = reinterpret_cast<unsigned short *>(win + kVhsWin + 8);         // walk: [kVhsJLevels][kVhsWin + 8]
+    __shared__ unsigned s_mat[31 * 31];
+    __shared__ unsigned s_cur[32]; // the generator state at the start of the next field
+    __shared__ int s_start, s_adv;
+    const int m = first + blockIdx.x, tid = threadIdx.x;
+    unsigned *raw = raw_base + (size_t) blockIdx.x * kVhsTailRaw;
+    if (tid < 32) s_cur[tid] = reinterpret_cast<const unsigned *>(&rands[m])[tid];
+    __syncthreads();
+    const int n = fields[blockIdx.x];
+    for (int f = 0; f < n; f++) {
+        vhs_apply(states[0], jump->field[ab], s_cur, tid, s_mat);
+        vhs_tail_stream(states, jump, raw, tid, s_mat);
+        int D = 0; // raw values consumed so far in the tail
+        for (int i0 = kVhsBulk; i0 < kInputSize;) {
+            const int line = i0 / kHres, xa = i0 - line * kHres;
+            const int fixed = vhs_fixed_draws(line);
+            const int e = kHres - ((xa == 0) ? 1 : xa); // regular samples of the line
+            vhs_line_tables(win, jt, &s_start, raw, D, i0, xa, line, fixed, tid);
+            if (tid == 0) { // the position after the line's last sample
+                int p = s_start;
+                if (fixed) {
+                    p += fixed * e;
+                } else {
+                    const unsigned short *far = jt + (kVhsJLevels - 1) * (kVhsWin + 8);
+                    for (int c = 0; c < (e >> (kVhsJLevels - 1)); c++) p = far[min(p, kVhsWin)];
+#pragma unroll
+                    for (int k = 0; k < kVhsJLevels - 1; k++)
+                        if ((e >> k) & 1) p = jt[k * (kVhsWin + 8) + min(p, kVhsWin)];
+                }
+                s_adv = p;
+            }
+            __syncthreads();
+            D += s_adv;
+            i0 += kHres - xa;
+            __syncthreads();
+        }
+        if (tid < 31) s_cur[tid] = raw[D - 31 + tid]; // D >= 31 always (the tail spans > 24 000 samples)
+        __syncthreads();
+    }
+    if (tid < 32) reinterpret_cast<unsigned *>(&rands_next[m])[tid] = (tid < 31) ? s_cur[tid] : 0u;
+}
 static_assert(kInputSize % kHres == 0, "the tail's per-line test assumes whole signal lines");
 
 } // namespace crt

@@ -259,6 +259,10 @@ static void vhs_build_jump(VhsJump *out)
         b = mat_mul(b, b);
         t = mat_mul(t, t);
     }
+    for (int ab = 0; ab < 2; ab++) { // k_vhs_skip: [aberration] + wobble + two draws per bulk sample
+        const Mat f = mat_pow(m, (unsigned) (ab + 1 + 2 * kVhsBulk));
+        memcpy(out->field[ab], f.data(), sizeof(out->field[ab]));
+    }
 }
 
 static void vhs_seed_state(unsigned seed, VhsRand *st)
@@ -879,6 +883,7 @@ int crtx_create(crtx_ctx **out, int n)
         CTX_TRY(cudaMalloc(&ctx->d_vhs_jump, sizeof(VhsJump)));
         CTX_TRY(cudaMalloc(&ctx->d_vhs_raw, sizeof(unsigned) * (size_t) kVhsTailRaw * n));
         CTX_TRY(cudaMalloc(&ctx->d_vhs_wants, sizeof(int) * n));
+        CTX_TRY(cudaMalloc(&ctx->d_vhs_fields, sizeof(int) * n));
         std::vector<VhsJump> j(1);
         vhs_build_jump(&j[0]);
         CTX_TRY(cudaMemcpy(ctx->d_vhs_jump, j.data(), sizeof(VhsJump), cudaMemcpyHostToDevice));
@@ -886,6 +891,7 @@ int crtx_create(crtx_ctx **out, int n)
         for (int i = 0; i < n; i++) vhs_seed_state(1u, &r[i]); // libc's default seed
         CTX_TRY(cudaMemcpy(ctx->d_vhs_rand, r.data(), sizeof(VhsRand) * n, cudaMemcpyHostToDevice));
         CTX_TRY(cudaFuncSetAttribute(k_noise_vhs, cudaFuncAttributeMaxDynamicSharedMemorySize, kVhsSmem));
+        CTX_TRY(cudaFuncSetAttribute(k_vhs_skip, cudaFuncAttributeMaxDynamicSharedMemorySize, kVhsSkipSmem));
     }
 #endif
     CTX_TRY(set_smem_attrs());
@@ -919,6 +925,7 @@ void crtx_destroy(crtx_ctx *ctx)
     cudaFree(ctx->d_vhs_jump);
     cudaFree(ctx->d_vhs_raw);
     cudaFree(ctx->d_vhs_wants);
+    cudaFree(ctx->d_vhs_fields);
     for (size_t i = 0; i < ctx->timed.size(); i++) {
         cudaEventDestroy(ctx->timed[i].start);
         cudaEventDestroy(ctx->timed[i].stop);
@@ -1041,6 +1048,65 @@ int crtx_seed(crtx_ctx *ctx, int first, int count, unsigned seed)
 #endif
     return 0;
 }
+
+#if (CRT_SYSTEM == CRT_SYSTEM_NTSCVHS)
+int crtx_get_rand(crtx_ctx *ctx, int first, int count, unsigned *words, void *stream)
+{
+    if (check_range(ctx, first, count)) return 1;
+    if (count == 0) return 0;
+    if (!words) return fail("crtx_get_rand: null words");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    std::vector<VhsRand> tmp(count);
+    CUDA_TRY(cudaMemcpyAsync(tmp.data(), static_cast<const VhsRand *>(ctx->d_vhs_rand) + first, sizeof(VhsRand) * count,
+                             cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    for (int i = 0; i < count; i++) memcpy(words + (size_t) i * CRTX_RAND_WORDS, tmp[i].hist, sizeof(tmp[i].hist));
+    return 0;
+}
+
+int crtx_set_rand(crtx_ctx *ctx, int first, int count, const unsigned *words, void *stream)
+{
+    if (check_range(ctx, first, count)) return 1;
+    if (count == 0) return 0;
+    if (!words) return fail("crtx_set_rand: null words");
+    std::vector<VhsRand> tmp(count);
+    for (int i = 0; i < count; i++) {
+        memcpy(tmp[i].hist, words + (size_t) i * CRTX_RAND_WORDS, sizeof(tmp[i].hist));
+        tmp[i].pad = 0;
+    }
+    // ordered on `stream` like crtx_set_state (pageable source: staged before the call returns)
+    CUDA_TRY(cudaMemcpyAsync(static_cast<VhsRand *>(ctx->d_vhs_rand) + first, tmp.data(), sizeof(VhsRand) * count,
+                             cudaMemcpyHostToDevice, static_cast<cudaStream_t>(stream)));
+    return 0;
+}
+
+int crtx_skip_fields(crtx_ctx *ctx, int first, int count, const int *fields, int do_aberration, void *stream)
+{
+    if (check_range(ctx, first, count)) return 1;
+    if (count == 0) return 0;
+    if (!fields) return fail("crtx_skip_fields: null fields");
+    for (int i = 0; i < count; i++)
+        if (fields[i] < 0) return fail("crtx_skip_fields: monitor %d: negative field count %d", first + i, fields[i]);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_vhs_fields + first, fields, sizeof(int) * count, cudaMemcpyHostToDevice, st));
+    k_vhs_skip<<<count, kVhsThreads, kVhsSkipSmem, st>>>(ctx->d_vhs_fields + first, static_cast<const VhsRand *>(ctx->d_vhs_rand),
+                                                         static_cast<VhsRand *>(ctx->d_vhs_rand_next),
+                                                         static_cast<const VhsJump *>(ctx->d_vhs_jump),
+                                                         ctx->d_vhs_raw + (size_t) first * kVhsTailRaw, do_aberration ? 1 : 0, first);
+    ctx->launches += 1;
+    k_vhs_commit<<<(count * 32 + 255) / 256, 256, 0, st>>>(static_cast<VhsRand *>(ctx->d_vhs_rand),
+                                                           static_cast<const VhsRand *>(ctx->d_vhs_rand_next), first, count);
+    ctx->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+#else
+// the builds without the replica: nothing draws from rand(), so there is no generator state to read, write or advance
+static int no_rand(const char *fn) { return fail("%s: this build draws no rand() (only the VHS build, CRT_SYSTEM_NTSCVHS, does)", fn); }
+int crtx_get_rand(crtx_ctx *, int, int, unsigned *, void *) { return no_rand("crtx_get_rand"); }
+int crtx_set_rand(crtx_ctx *, int, int, const unsigned *, void *) { return no_rand("crtx_set_rand"); }
+int crtx_skip_fields(crtx_ctx *, int, int, const int *, int, void *) { return no_rand("crtx_skip_fields"); }
+#endif
 
 signed char *crtx_analog(crtx_ctx *ctx, int i)
 {

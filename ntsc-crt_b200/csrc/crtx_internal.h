@@ -55,6 +55,7 @@ struct crtx_ctx {
     void *d_vhs_jump = nullptr;   // VHS: jump-ahead matrices
     unsigned *d_vhs_raw = nullptr; // VHS: tail raw-stream scratch
     int *d_vhs_wants = nullptr;   // VHS: do_aberration flags of the current modulate
+    int *d_vhs_fields = nullptr;  // VHS: field counts of the current crtx_skip_fields
     bool vhs_seeded = false;
     int vhs_draw_aberration = 0;
     unsigned char *d_src_img = nullptr; // crtx_frames_host staging, src_slot bytes per monitor

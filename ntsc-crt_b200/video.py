@@ -22,6 +22,18 @@ sequential loop, which tests/test_gpu_video.py checks against the oracle.
 
 Frames shard across ranks the same way (`sharding.shard_range`); the cross-rank check needs the previous
 rank's final state and last image, exchanged with one small all_gather.
+
+The VHS build (video_convert.c built with CRT_SYSTEM_NTSCVHS) carries less and one thing more:
+
+    hsync, ccf, rn  -> reset by every crt_modulate (crt_ntscvhs.c:259, 332-336) or overwritten by rand()
+                       before use (crt_core.c:349): nothing to carry, and hsync is not compared
+    vsync           -> speculated, then verified, as above
+    rand() state    -> a pure function of the seed, the frame index and do_aberration (a field's draw count
+                       depends on its own draws only): each segment's monitor is seeded and advanced to its
+                       first decoded frame with crtx_skip_fields, so it is exact, never speculated
+
+The generator state after a segment's halo is saved, and a repair restores it before redoing the segment.
+Each rank computes its own segments' states from the seed, so nothing about rand() is exchanged.
 """
 import ctypes as C
 
@@ -57,17 +69,24 @@ def frame_parity(f, progressive=False):
 
 class VideoConverter:
     def __init__(self, variant="ntsc", outw=640, outh=480, noise=12, scanlines=1, as_color=1,
-                 progressive=False, segments=64, fmt=layout.PIX_BGRA, saturation=10, batch_factory=None):
+                 progressive=False, segments=64, fmt=layout.PIX_BGRA, saturation=10, batch_factory=None, seed=1,
+                 do_aberration=0):
         """batch_factory(variant, n) -> an object with capi.Batch's interface (default: capi.Batch itself, the CUDA
         library).  The CPU test-suite injects an oracle-backed stand-in to exercise the scheduling logic below
-        (tests/mock_batch.py); nothing else ever should."""
+        (tests/mock_batch.py); nothing else ever should.
+
+        VHS variants only: the sequence is the one srand(seed) followed by video_convert.c's loop gives, with
+        do_aberration set in its settings (its -a flag)."""
         import torch
         self.torch = torch
         self._factory = batch_factory if batch_factory is not None else capi.Batch
         self._pool = {}  # monitors are kept between convert() calls: creating and freeing a context costs tens of ms
         self.variant, self.spec = variant, layout.system_spec(variant)
-        if self.spec.system != layout.SYS_NTSC:
-            raise ValueError("the video path covers CRT_SYSTEM_NTSC (what video_convert.c is built for)")
+        if self.spec.system not in (layout.SYS_NTSC, layout.SYS_VHS):
+            raise ValueError("the video path covers CRT_SYSTEM_NTSC and CRT_SYSTEM_NTSCVHS (what video_convert.c is built for)")
+        self.vhs = self.spec.system == layout.SYS_VHS
+        self.seed, self.do_aberration = seed, (1 if do_aberration else 0)
+        self._extra = dict(do_aberration=self.do_aberration) if self.vhs else {}  # per-field source settings
         self.outw, self.outh, self.noise, self.fmt = outw, outh, noise, fmt
         self.knobs = dict(blend=0, scanlines=scanlines, saturation=saturation)  # video_convert.c:239-241
         self.as_color, self.progressive = as_color, progressive
@@ -98,7 +117,7 @@ class VideoConverter:
         for f in range(lo, hi):
             field, frame = frame_parity(first_frame + f, self.progressive)
             b.set_source(i, frames[f], format=self.fmt, as_color=self.as_color, field=field, frame=frame,
-                         raw=0, hue=0, xoffset=0, yoffset=0)
+                         raw=0, hue=0, xoffset=0, yoffset=0, **self._extra)
             b.modulate(first=i, count=1)
             b.demodulate(first=i, count=1)
             outputs[f].copy_(self._work[i])
@@ -151,10 +170,13 @@ class VideoConverter:
         fresh = (capi.State * 1)()  # what crt_init leaves (crt_core.c:250-269): the probe monitor may have been used before
         fresh[0].hsync, fresh[0].vsync, fresh[0].rn = 0, 0, 194
         probe.set_state(fresh)
+        if self.vhs:  # the generator the sequence has at this rank's first frame
+            probe.seed(self.seed, first=0, count=1)
+            probe.skip_fields([first_frame], self.do_aberration)
         after = {}
         for f in range(min(4, n)):
             field, frame = frame_parity(first_frame + f, self.progressive)
-            probe.set_source(0, frames[f], format=self.fmt, as_color=self.as_color, field=field, frame=frame)
+            probe.set_source(0, frames[f], format=self.fmt, as_color=self.as_color, field=field, frame=frame, **self._extra)
             probe.modulate()
             probe.demodulate()
             st = probe.get_state()[0]
@@ -175,6 +197,9 @@ class VideoConverter:
                 hs, vs = after.get((halo0[s] - 1) & 1, (0, 0))  # speculation: state after frame halo0 - 1
             states[s].hsync, states[s].vsync, states[s].rn = hs, vs, rn_before(halo0[s])
         b.set_state(states)
+        if self.vhs:  # every segment's generator where the sequential loop has it before frame halo0[s]
+            b.seed(self.seed, first=0, count=S)
+            b.skip_fields(halo0, self.do_aberration)
 
         # the settings table of the batch as numpy columns (the CUDA library's Batch; the CPU test double has none)
         table = capi.source_table(b.sources) if hasattr(b, "sources") else None
@@ -183,6 +208,8 @@ class VideoConverter:
             import numpy as np
             table["format"], table["as_color"], table["raw"], table["hue"] = self.fmt, self.as_color, 0, 0
             table["xoffset"], table["yoffset"] = 0, 0
+            if self.vhs:
+                table["do_aberration"] = self.do_aberration
             table["h"], table["w"] = frames.shape[1], frames.shape[2]
             base_mine = frames.data_ptr()
             base_prev = prev_in.data_ptr() if prev_in is not None else 0
@@ -206,7 +233,7 @@ class VideoConverter:
                 for s, gf in items:
                     field, frame = frame_parity(gf, self.progressive)
                     b.set_source(s, src_frame(gf), format=self.fmt, as_color=self.as_color, field=field, frame=frame,
-                                 raw=0, hue=0, xoffset=0, yoffset=0)
+                                 raw=0, hue=0, xoffset=0, yoffset=0, **self._extra)
             b.modulate(first=lo_s, count=len(items))
             b.demodulate(first=lo_s, count=len(items))
 
@@ -214,6 +241,10 @@ class VideoConverter:
         step([(s, starts[s] - 1) for s in range(S) if starts[s] >= 1])
         st_halo = [(x.hsync, x.vsync) for x in b.get_state()]
         halo_img = {s: self._work[s].clone() for s in range(S) if starts[s] >= 1}
+        rand_halo = b.get_rand(0, S) if self.vhs else None  # exact: the halo's draws do not depend on its sync state
+
+        def same_sync(x, y):  # VHS: the next modulate resets hsync, so only vsync carries over
+            return x[1] == y[1] if self.vhs else x == y
 
         # ---- main steps: step t advances every segment still inside its span by one frame; shard_range puts
         # the longer segments first, so the active ones are always 0 .. count-1
@@ -251,9 +282,9 @@ class VideoConverter:
                 pl = outputs[spans[s - 1][1] - 1] if s > 0 else prev_last
                 if pf is None:
                     continue
-                if s in basis and basis[s][0] == pf and bool(torch.equal(basis[s][1], pl)):
+                if s in basis and same_sync(basis[s][0], pf) and bool(torch.equal(basis[s][1], pl)):
                     continue  # already exact against this very predecessor
-                if s not in repaired and st_halo[s] == pf and bool(torch.equal(halo_img[s], pl)):
+                if s not in repaired and same_sync(st_halo[s], pf) and bool(torch.equal(halo_img[s], pl)):
                     if world > 1:
                         basis[s] = (pf, pl.clone())
                     continue  # the speculation held
@@ -267,6 +298,8 @@ class VideoConverter:
                 redo = (capi.State * 1)()
                 redo[0].hsync, redo[0].vsync, redo[0].rn = pf[0], pf[1], rn_before(first_frame + a)
                 b.set_state(redo, first=s)
+                if self.vhs:
+                    b.set_rand(rand_halo[s:s + 1], first=s)
                 self._work[s].copy_(pl)
                 self._run_sequential(b, s, frames, a, e, outputs, first_frame)
                 x = b.get_state(first=s, count=1)[0]

@@ -22,18 +22,34 @@
  * A segment that fails verification is decoded again, sequentially, from the true state; its
  * files are rewritten.  The result is what the sequential loop writes (tests/test_gpu_video_driver.py).
  *
+ * Linked against the VHS library (crtx_system() says so at run time) it is video_convert.c's VHS build.  There the
+ * noise comes from rand(): the sequence is srand(seed) followed by the loop, and every segment's generator is made
+ * exact from the seed (crtx_seed, then crtx_skip_fields to its first image), saved after the halo and restored when
+ * the segment is redone.  hsync is reset by every crt_modulate of that build (crt_ntscvhs.c:259), so only vsync and
+ * the image are verified.
+ *
  *   cc -std=c89 -O2 -pthread -I../include crtx_video.c -L../ntsc-crt_b200/lib -lcrt_b200_ntsc -o crtx_video
- *   ./crtx_video [-m] [-p] [-a] [-S segments] num_frames outwidth outheight noise
- * (-m monochrome, -p progressive, -a no scanlines: the letters of video_convert.c's option word.)
+ *   ./crtx_video [-m] [-p] [-a] [-s] [-S segments] [-R seed] num_frames outwidth outheight noise
+ * (-m monochrome, -p progressive, -s no scanlines: the letters of video_convert.c's option word; -a is no scanlines
+ * too, except on the VHS build, where it draws the aberration as video_convert.c's -a does.  -R: the rand() seed of
+ * the VHS build, time(0) by default as in video_convert.c:218; the seed used is printed.)
  */
 #include <pthread.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <time.h>
 
 #include "crtx_batch.h"
 
 #define PIX_BGRA 5 /* CRT_PIX_FORMAT_BGRA, crt_core.h:67 */
+#define SYSTEM_NTSCVHS 5 /* CRT_SYSTEM_NTSCVHS, crt_core.h:35 */
+
+/* 1 for crtx_video_vhs (tools/Makefile): the generator calls of crtx_batch.h are linked in, and used when the library
+ * says at run time that it is the VHS build.  The NTSC binary references none of them. */
+#ifndef CRTX_VIDEO_VHS
+#define CRTX_VIDEO_VHS 0
+#endif
 
 static void
 die(const char *what)
@@ -115,6 +131,21 @@ bmp_save(const char *file, const unsigned char *file_pixels, int w, int h)
     return 1;
 }
 
+/* ---- the VHS build's rand() replica: seed, skip to each segment's first image, save and restore ---- */
+#if CRTX_VIDEO_VHS
+static int build_is_vhs(void) { return crtx_system() == SYSTEM_NTSCVHS; }
+static void rand_seed(crtx_ctx *c, int n, unsigned seed) { TRY(crtx_seed(c, 0, n, seed)); }
+static void rand_skip(crtx_ctx *c, int n, const int *fields, int ab) { TRY(crtx_skip_fields(c, 0, n, fields, ab, NULL)); }
+static void rand_get(crtx_ctx *c, int n, unsigned *words) { TRY(crtx_get_rand(c, 0, n, words, NULL)); }
+static void rand_set(crtx_ctx *c, int i, const unsigned *words) { TRY(crtx_set_rand(c, i, 1, words, NULL)); }
+#else
+static int build_is_vhs(void) { return 0; }
+static void rand_seed(crtx_ctx *c, int n, unsigned seed) { (void) c; (void) n; (void) seed; }
+static void rand_skip(crtx_ctx *c, int n, const int *fields, int ab) { (void) c; (void) n; (void) fields; (void) ab; }
+static void rand_get(crtx_ctx *c, int n, unsigned *words) { (void) c; (void) n; (void) words; }
+static void rand_set(crtx_ctx *c, int i, const unsigned *words) { (void) c; (void) i; (void) words; }
+#endif
+
 /* ---- n steps of rn = 214019 * rn + 140327895 (crt_core.c:359) as one multiply-add ---- */
 static unsigned
 lcg_advance(unsigned rn, unsigned long n)
@@ -151,6 +182,7 @@ struct job {
     int n;              /* images: files 1 .. n, image index f = file number - 1 */
     int outw, outh, noise;
     int color, progressive, scanlines;
+    int vhs, aberration; /* VHS build; its -a */
     int w, h;           /* source size (all images alike) */
     int bits;           /* of the source files: 24 or 32 */
     size_t src_bytes, out_bytes, file_bytes; /* device image, device output, source pixel array as stored */
@@ -256,6 +288,7 @@ fill_source(const struct job *j, crtx_source *s, const void *dev, int f)
     s->w = j->w;
     s->h = j->h;
     s->as_color = j->color;
+    s->do_aberration = j->aberration;
     parity_of(j, f, &s->field, &s->frame);
 }
 
@@ -274,11 +307,15 @@ main(int argc, char **argv)
     void **dsrc, **draw, **dfile, **work, **halo;
     int after_hs[2], after_vs[2], have_after[2];
     unsigned rn0 = 194u; /* crt_init, crt_core.c:269 */
+    unsigned seed = (unsigned) time(0);
+    unsigned *rand_halo = NULL; /* VHS: every segment's generator after its halo, CRTX_RAND_WORDS words each */
+    int *skip = NULL;
     char name[64];
 
     memset(&j, 0, sizeof(j));
     j.color = 1;
     j.scanlines = 1;
+    j.vhs = build_is_vhs();
     while (a < argc && argv[a][0] == '-') {
         const char *o = argv[a] + 1;
         if (*o == 'S' && a + 1 < argc) {
@@ -286,9 +323,16 @@ main(int argc, char **argv)
             a += 2;
             continue;
         }
+        if (*o == 'R' && a + 1 < argc) {
+            seed = (unsigned) strtoul(argv[a + 1], NULL, 0);
+            a += 2;
+            continue;
+        }
         for (; *o; o++) {
             if (*o == 'm') j.color = 0;
             else if (*o == 'p') j.progressive = 1;
+            else if (*o == 's') j.scanlines = 0;
+            else if (*o == 'a' && j.vhs) j.aberration = 1;
             else if (*o == 'a') j.scanlines = 0;
             else if (*o != 'o') {
                 fprintf(stderr, "crtx_video: unknown option -%c\n", *o);
@@ -298,7 +342,7 @@ main(int argc, char **argv)
         a++;
     }
     if (argc - a < 4) {
-        fprintf(stderr, "usage: %s [-m] [-p] [-a] [-S segments] num_frames outwidth outheight noise\n", argv[0]);
+        fprintf(stderr, "usage: %s [-m] [-p] [-a] [-s] [-S segments] [-R seed] num_frames outwidth outheight noise\n", argv[0]);
         return EXIT_FAILURE;
     }
     j.n = atoi(argv[a]) - 1; /* the reference converts files 1 .. num_frames - 1 (video_convert.c:246) */
@@ -336,6 +380,8 @@ main(int argc, char **argv)
     S = segments < j.n ? segments : j.n;
     lo = (int *) malloc(sizeof(int) * S);
     hi = (int *) malloc(sizeof(int) * S);
+    skip = (int *) malloc(sizeof(int) * S);
+    rand_halo = (unsigned *) malloc(sizeof(unsigned) * CRTX_RAND_WORDS * S);
     mons = (crtx_monitor *) calloc(S, sizeof(*mons));
     srcs = (crtx_source *) calloc(S, sizeof(*srcs));
     st = (crtx_state *) calloc(S, sizeof(*st));
@@ -350,7 +396,7 @@ main(int argc, char **argv)
     dfile = (void **) calloc(S, sizeof(*dfile));
     work = (void **) calloc(S, sizeof(*work));
     halo = (void **) calloc(S, sizeof(*halo));
-    if (!lo || !hi || !mons || !srcs || !st || !st_halo || !fin || !hsrc || !hout || !hsrc2 || !hout2 || !dsrc || !draw || !dfile || !work || !halo) die("out of memory");
+    if (!lo || !hi || !skip || !rand_halo || !mons || !srcs || !st || !st_halo || !fin || !hsrc || !hout || !hsrc2 || !hout2 || !dsrc || !draw || !dfile || !work || !halo) die("out of memory");
 
     TRY(crtx_create(&ctx, S));
     longest = 0;
@@ -380,6 +426,7 @@ main(int argc, char **argv)
     }
     TRY(crtx_set_monitors(ctx, 0, S, mons));
     printf("converting %d images %dx%d -> %dx%d in %d segments...\n", j.n, j.w, j.h, j.outw, j.outh, S);
+    if (j.vhs) printf("rand() seed %u\n", seed);
 
     /* ---- what a steady decode holds after an image of each parity: a 4-image probe, noise 0 ---- */
     have_after[0] = have_after[1] = 0;
@@ -394,6 +441,7 @@ main(int argc, char **argv)
         pm.noise = 0;
         TRY(crtx_create(&probe, 1));
         TRY(crtx_set_monitors(probe, 0, 1, &pm));
+        if (j.vhs) rand_seed(probe, 1, seed);
         for (f = 0; f < 4 && f < j.n; f++) {
             stage_image(&j, f, hsrc[0], draw[0], dsrc[0]);
             fill_source(&j, &ps, dsrc[0], f);
@@ -417,8 +465,13 @@ main(int argc, char **argv)
             st[s].vsync = after_vs[(h0 - 1) & 1];
         }
         st[s].rn = as_int32(lcg_advance(rn0, (unsigned long) crtx_input_size() * (unsigned long) h0));
+        skip[s] = h0;
     }
     TRY(crtx_set_state(ctx, 0, S, st, NULL));
+    if (j.vhs) { /* every segment's generator where the sequential loop has it before image h0 */
+        rand_seed(ctx, S, seed);
+        rand_skip(ctx, S, skip, j.aberration);
+    }
 
     /* ---- halo: images lo - 2 and lo - 1 (segments that have them are a suffix of the list) ---- */
     for (t = 2; t >= 1; t--) {
@@ -437,6 +490,7 @@ main(int argc, char **argv)
         TRY(crtx_sync(NULL)); /* the pinned staging buffers are reused by the next step */
     }
     TRY(crtx_get_state(ctx, 0, S, st_halo, NULL));
+    if (j.vhs) rand_get(ctx, S, rand_halo); /* exact: the halo's draws do not depend on its sync state */
     for (s = 1; s < S; s++) TRY(crtx_memcpy(halo[s], work[s], j.out_bytes, 2, NULL));
 
     /* ---- main steps: step t decodes image lo[s] + t of every segment still inside its span; longer
@@ -514,7 +568,7 @@ main(int argc, char **argv)
     /* ---- verification in sequence order; a failed segment is redone from the true state ---- */
     for (s = 1; s < S; s++) {
         int differ = 0, f;
-        if (st_halo[s].hsync == fin[s - 1].hsync && st_halo[s].vsync == fin[s - 1].vsync) {
+        if ((j.vhs || st_halo[s].hsync == fin[s - 1].hsync) && st_halo[s].vsync == fin[s - 1].vsync) {
             TRY(crtx_memcmp_device(halo[s], work[s - 1], j.out_bytes, &differ, NULL));
             if (!differ) continue;
         }
@@ -524,6 +578,7 @@ main(int argc, char **argv)
         st[s].vsync = fin[s - 1].vsync;
         st[s].rn = as_int32(lcg_advance(rn0, (unsigned long) crtx_input_size() * (unsigned long) lo[s]));
         TRY(crtx_set_state(ctx, s, 1, &st[s], NULL));
+        if (j.vhs) rand_set(ctx, s, rand_halo + (size_t) s * CRTX_RAND_WORDS);
         TRY(crtx_memcpy(work[s], work[s - 1], j.out_bytes, 2, NULL));
         for (f = lo[s]; f < hi[s]; f++) {
             stage_image(&j, f, hsrc[s], draw[s], dsrc[s]);
@@ -550,5 +605,7 @@ main(int argc, char **argv)
         crtx_device_free(halo[s]);
     }
     crtx_destroy(ctx);
+    free(skip);
+    free(rand_halo);
     return EXIT_SUCCESS;
 }
