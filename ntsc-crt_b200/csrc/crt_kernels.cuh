@@ -362,7 +362,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb(const SrcCfg *__rest
     picture_size(s, destw, desth);
     if (destw <= 0 || desth <= 0 || s.w <= 0 || s.h <= 0) return;
     picture_origin(s, destw, desth, xo, yo);
-    const int white = kWhite * cfg.white_point / 100;
+    const int white = white_scale(cfg.white_point);
     const int ire0 = kBlack + cfg.black_point;
     int rp, gp, bp;
     fmt_positions(s.format, rp, gp, bp);
@@ -563,7 +563,7 @@ __global__ void __launch_bounds__(256, 2) k_mod_picture_rgb_staged(const SrcCfg 
     __syncwarp();
     int xo, yo;
     picture_origin(s, destw, desth, xo, yo);
-    const int white = kWhite * cfg.white_point / 100;
+    const int white = white_scale(cfg.white_point);
     const int ire0 = kBlack + cfg.black_point;
     const unsigned char *data = static_cast<const unsigned char *>(s.data);
     constexpr bool color = COLOR;
@@ -846,7 +846,10 @@ __global__ void CRT_NES_MOD_BOUNDS k_mod_nes(const SrcCfg *__restrict__ srcs, co
                 analog[n * kHres + t] = nes_border_sample(tab, nes_border_color(&srcs[m]), n, s.dot_crawl_offset, t);
             }
         }
-        if (tid < kBurstLen) { // crt_nes.c:174-178
+        // crt_nes.c:174-178.  The reference writes the burst before the picture, so where a picture that starts before
+        // the burst's end covers it (xoffset < CB_BEG + burst - AV_BEG) the picture's bytes stand: those burst bytes are
+        // not stored, since the threads writing the two are not ordered
+        if (tid < kBurstLen && (kCbBeg + tid < xo || kCbBeg + tid >= xo + kAvLen)) {
             const int t = kCbBeg + tid;
             analog[n * kHres + t] = burst[(n % 3) * 4 + (t & 3)];
         }
@@ -936,7 +939,7 @@ __global__ void __launch_bounds__(256) k_mod_snes(const SrcCfg *__restrict__ src
     int destw, desth, xo, yo;
     picture_size(s, destw, desth);
     picture_origin(s, destw, desth, xo, yo);
-    const int white = kWhite * cfg.white_point / 100;
+    const int white = white_scale(cfg.white_point);
     const int ire0 = kBlack + cfg.black_point;
     const unsigned char *data = static_cast<const unsigned char *>(s.data);
 
@@ -1002,7 +1005,7 @@ __global__ void __launch_bounds__(256, 8) k_mod_nesrgb(const SrcCfg *__restrict_
     __syncthreads();
 
     const int xo = (kAvBeg + s.xoffset) & ~3, yo = kTop + s.yoffset; // crt_nesrgb.c:86-90
-    const int white = kWhite * cfg.white_point / 100;
+    const int white = white_scale(cfg.white_point);
     const int ire0 = kBlack + cfg.black_point;
     const unsigned char *data = static_cast<const unsigned char *>(s.data);
 
@@ -1015,7 +1018,7 @@ __global__ void __launch_bounds__(256, 8) k_mod_nesrgb(const SrcCfg *__restrict_
         const int y = n - yo;
         if (bpp == 0 || y < 0 || y >= kLines || s.h <= 0 || s.w <= 0) continue;
         if (s.reinit) __syncthreads(); // (block-uniform) template before burst and picture
-        if (tid < kBurstLen) { // crt_nesrgb.c:104-110
+        if (tid < kBurstLen && (kCbBeg + tid < xo || kCbBeg + tid >= xo + kAvLen)) { // crt_nesrgb.c:104-110 (as k_mod_nes)
             const int t = kCbBeg + tid;
             line[t] = burst_byte(burst[n % kVper][t & 3]);
         }

@@ -382,8 +382,9 @@ __global__ void __launch_bounds__(kSyncThreads, 2) k_sync(const MonCfg *__restri
         }
     }
     // |bright| bound of the fast equaliser path (crt_lines.cuh); halved for the PV-1000, whose luma cascade
-    // (hf = 80024) is only proven wrap-free up to there
-    if (tid == 0) sh.generic = force_generic || abs(cfg.brightness - (kBlack + cfg.black_point)) > (kCc == 5 ? 2048 : 4096);
+    // (hf = 80024) is only proven wrap-free up to there.  bright wraps as in the reference (crt_core.c:304), and its
+    // magnitude is taken in 64 bits: abs(INT_MIN) is INT_MIN, which would pass the bound
+    if (tid == 0) sh.generic = force_generic || llabs((long long) wsub(cfg.brightness, wadd(kBlack, cfg.black_point))) > (kCc == 5 ? 2048 : 4096);
     __syncthreads();
     phase_mark(0, 1);
 

@@ -88,6 +88,14 @@ constexpr int kBurstLen = CB_CYCLES * CRT_CB_FREQ;
 constexpr int kDestW = kBloom ? (kAvLen * 55500) >> 16 : kAvLen;
 constexpr int kDestH = kBloom ? ((CRT_BOT - CRT_TOP) * 63500) >> 16 : ((CRT_BOT - CRT_TOP) * 64500) >> 16;
 constexpr int kWhite = WHITE_LEVEL;
+// The white scale WHITE_LEVEL * white_point / 100 of the RGB encoders (crt_ntsc.c:318; the same line in crt_ntscvhs.c,
+// crt_snes.c, crt_template.c, crt_pv1k.c and crt_nesrgb.c).  Signed overflow being undefined, gcc -O3 folds the
+// expression to white_point where WHITE_LEVEL is 100 -- every system that computes it -- so the compiled reference's
+// scale is white_point itself, also where 100 * white_point would wrap.  Any other level wraps like the reference's
+// multiplication.
+__host__ __device__ constexpr int white_scale(int white_point) {
+    return kWhite == 100 ? white_point : (int) ((unsigned) kWhite * (unsigned) white_point) / 100;
+}
 constexpr int kBurst = BURST_LEVEL;
 constexpr int kBlack = BLACK_LEVEL;
 constexpr int kBlank = BLANK_LEVEL;

@@ -21,6 +21,15 @@ static i32 wadd(i32 a, i32 b) { return (i32) ((u32) a + (u32) b); }
 static i32 wsub(i32 a, i32 b) { return (i32) ((u32) a - (u32) b); }
 static i32 posmod(i32 x, i32 n) { return ((x % n) + n) % n; } /* crt_core.c:17 */
 
+/* WHITE_LEVEL * white_point / 100, the white scale of the RGB encoders (crt_ntsc.c:318 and the same line of every
+ * other RGB encoder).  Signed overflow being undefined, gcc -O3 folds it to white_point where WHITE_LEVEL is 100 --
+ * every system that computes it -- so the compiled reference does not wrap 100 * white_point there. */
+static i32
+white_scale(const ocrt_sys *sys, i32 white_point)
+{
+    return sys->white_level == 100 ? white_point : wmul(sys->white_level, white_point) / 100;
+}
+
 /* ------------------------------------------------------------------------- */
 /* fixed-point trigonometry (crt_core.c:19-61)                               */
 /* ------------------------------------------------------------------------- */
@@ -512,7 +521,7 @@ ocrt_encode_rgb(const ocrt_sys *sys, ocrt_monitor *m, ocrt_rgb_source *src, ocrt
     if (sys->system == OCRT_SYS_VHS) m->hsync = 0; /* crt_ntscvhs.c:258-259 */
 
     /* picture (crt_ntsc.c:254-324) */
-    white = sys->white_level * m->white_point / 100;
+    white = white_scale(sys, m->white_point);
     for (y = 0; y < desth; y++) {
         i32 hy = 0, hi = 0, hq = 0;
         i32 row = (y * src->h) / desth + (src->field * src->h + desth) / desth / 2;
@@ -610,7 +619,7 @@ encode_template_family(const ocrt_sys *sys, ocrt_monitor *m, ocrt_rgb_source *sr
         }
     }
 
-    white = sys->white_level * m->white_point / 100;
+    white = white_scale(sys, m->white_point);
     for (y = 0; y < desth; y++) { /* crt_snes.c:252-320 */
         i32 hy = 0, hi = 0, hq = 0; /* reset_iir per line */
         i32 row = (y * src->h) / desth, ph = (y + yo) % V;
@@ -700,7 +709,7 @@ ocrt_encode_nesrgb(const ocrt_sys *sys, ocrt_monitor *m, ocrt_nesrgb_source *src
     if (bpp == 0) return; /* crt_nesrgb.c:81-84 */
     xo = (sys->av_beg + src->xoffset) & ~3;
     yo = sys->top + src->yoffset;
-    white = sys->white_level * m->white_point / 100;
+    white = white_scale(sys, m->white_point);
 
     for (y = 0; y < sys->lines; y++) { /* crt_nesrgb.c:92-164 */
         signed char *line = m->analog + (y + yo) * H;

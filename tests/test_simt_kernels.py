@@ -28,6 +28,7 @@ import test_gpu_fullsize as _fullsize  # noqa: E402
 import test_gpu_fuzz as _fuzz  # noqa: E402
 import test_gpu_guard_edges as _guard  # noqa: E402
 import test_gpu_inp_elision as _elision  # noqa: E402
+import test_gpu_knob_domain as _knob  # noqa: E402
 import test_gpu_lines2 as _lines2  # noqa: E402
 import test_gpu_lineshard as _lineshard  # noqa: E402
 import test_gpu_parity as _parity  # noqa: E402
@@ -109,6 +110,7 @@ _adopt(_api, "api")
 _adopt(_guard, "guard")
 _adopt(_vfac, "vfac")
 _adopt(_vhs, "vhs")
+_adopt(_knob, "knob")
 test_cli_unmodified_cli_driver_is_byte_identical = _cli.test_unmodified_cli_driver_is_byte_identical
 _adopt(_still, "still")
 test_vconv_unmodified_video_convert_runs_against_the_library = _vconv.test_unmodified_video_convert_runs_against_the_library
@@ -134,6 +136,19 @@ def small_vhs_runs(monkeypatch):
     monkeypatch.setattr(_vhs, "FIELDS", 3)
     monkeypatch.setattr(_vhs, "SWEEP_CASES", 1)
     monkeypatch.setattr(_vhs, "SWEEP_CALLS", 2)
+
+
+@pytest.fixture(autouse=True)
+def small_knob_tables(monkeypatch):
+    """tests/test_gpu_knob_domain.py with every fourth case of each variant's table (the GPU runs all of them)"""
+    monkeypatch.setattr(_knob, "CASES", 4)
+
+
+@pytest.mark.parametrize("variant", ["ntsc", "nes", "pv1k"])
+def test_knob_dropin_whole_table(variant, monkeypatch):
+    """the whole knob-domain table through the drop-in, on one variant of each encoder family"""
+    monkeypatch.setattr(_knob, "CASES", None)
+    _knob.test_dropin_knob_domain(variant)
 
 
 _BFUZZ_FULL = dict(MAX_MONITORS=_bfuzz.MAX_MONITORS, FIELDS=_bfuzz.FIELDS, MAX_OUTW=_bfuzz.MAX_OUTW)
